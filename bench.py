@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Driver benchmark for the B200-native quantized-linear hot path.
+"""Benchmark of the H100-native quantized-linear hot path.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME] [--no-extras]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME] [--no-extras] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic input.  The default workload is the configuration
 BASELINE.json's metric is quoted on (configs[1]): the bf16 x int4 QLinear GEMM M=4096, K=4096, N=14336 (Llama-3-8B FFN
@@ -54,6 +54,7 @@ DEFAULT_WORKLOAD = "qlinear_bf16_int4_m4096"
 EXTRA_WORKLOADS = ["decode_m1", "decode_m8", "decode_m32", "int8_m4096", "llama3_8b_decode_b1", "llama3_8b_decode_b8",
                    "llama3_8b_decode_b32"]
 EXTRA_WORKLOADS_MULTI = ["decode_m1", "decode_m8", "llama3_8b_decode_b1", "llama3_8b_decode_b8"]
+DUMP_ROWS = 1024  # --dump-outputs: at most 1024 x 14336 float32 = 59 MB
 
 
 def load_peaks():
@@ -62,7 +63,7 @@ def load_peaks():
         p = json.load(open(path))
         return dict(hbm=p["hbm_gbs"], tensor=p["bf16_tflops"], tensor_sustained=p.get("bf16_tflops_sustained"),
                     source="measured (MEASURED_PEAKS.json, burst)")
-    return dict(hbm=6650.0, tensor=1590.0, tensor_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm=3350.0, tensor=989.0, tensor_sustained=None, source="H100 SXM data sheet (dense bf16, 700 W)")
 
 
 def algorithmic(kind, M, N, K):
@@ -87,7 +88,7 @@ def metric_name(workload):
 
 
 class ClockSampler:
-    """Samples SM clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe).
+    """Samples SM clocks / throttle reasons DURING the timed region.
 
     NVML is read in-process from a thread (pynvml, ~0.1 ms per sample, every 2 ms); the timed regions of the default
     workload last only a few milliseconds, less than `nvidia-smi -lms` needs to print its first line.  Falls back to
@@ -473,7 +474,7 @@ class Bench:
         n_local = N_DIM // world
         mark = self.sampler.n_samples()
         # resident state: the local weight shard; several rotated copies for the HBM-bound decode shapes so that the
-        # packed weights are re-read from HBM, not from the 126 MB L2
+        # packed weights are re-read from HBM, not from the 50 MB L2
         n_copies = 1 if not hbm else max(2, int(160e6 // (n_local * K_DIM // 2)) + 1)
         if kind == "int4":
             fulls = [make_int4(N_DIM, K_DIM, dev, seed=1000 + c) for c in range(n_copies)]  # same on every rank
@@ -537,14 +538,16 @@ class Bench:
                 graphs.append(gr)
             rotation = torch.cuda.CUDAGraph()
             with torch.cuda.graph(rotation):
-                for c in range(n_copies):
-                    gathered(x_dev, weights[c])
+                rotation_outs = [gathered(x_dev, weights[c]) for c in range(n_copies)]
+
+        last_out = [None]  # what the last device-timed step returned (--dump-outputs)
 
         def step_device(i):
             if graphs is not None:
                 graphs[i % n_copies].replay()
                 return graph_outs[i % n_copies]
-            return gathered(x_dev, weights[i % n_copies])
+            last_out[0] = gathered(x_dev, weights[i % n_copies])
+            return last_out[0]
 
         pipe = None
         if not hbm and world == 1:
@@ -576,6 +579,9 @@ class Bench:
             ms_dev = self.timed(run_steps, 1, self.warm) / steps
         else:
             ms_dev = self.timed(step_device, steps, self.warm)
+        if name == args.workload and args.dump_outputs:
+            # the output buffer of the last timed step: a single-step graph's, the rotation graph's last, or the eager one
+            self.dump_output((graph_outs[rest - 1] if rest else rotation_outs[-1]) if rotation is not None else last_out[0])
         ms_e2e = self.timed(step_e2e, steps, self.warm)
         # roofline of the dominant kernel: the local shard's kernel alone (no gather), CUDA events on the launching stream
         if world == 1:
@@ -602,23 +608,19 @@ class Bench:
             achieved, peak, peak_src = flops_l / (ms_kernel * 1e-3) / 1e12, self.peaks["tensor"], self.peaks["source"]
             if kind == "int8":
                 peak, peak_src = self.int8_peak()
-        traffic = None
-        prof = os.path.join(ROOT, "profiles", "traffic.json")
-        if world == 1 and os.path.exists(prof):  # measured once under ncu for the single-GPU kernel; meaningless per shard
-            traffic = json.load(open(prof)).get(name)
         res = {
             "metric": metric_name(name), "value": scale_f(ms_dev), "unit": unit, "ms_per_step": ms_dev,
             "dtype": "bf16" if kind == "int4" else "int8",
             "config": {"workload": name, "M": M, "N": N_DIM, "K": K_DIM, "group_size": GROUP,
                        "weights": "qint4 canonical packing" if kind == "int4" else "qint8",
                        "parallelism": self.parallelism_note(fg is not None),
-                       "l2": ("inputs larger than L2 (A+W+out = %.0f MB > 126 MB)" % (byts / 1e6)) if not hbm else
+                       "l2": ("inputs larger than L2 (A+W+out = %.0f MB > 50 MB)" % (byts / 1e6)) if not hbm else
                              f"{n_copies} rotated weight copies ({n_copies * n_local * K_DIM // 2 / 1e6:.0f} MB > L2)",
                        **({"launch": "CUDA graph replay (one kernel per step)"} if graphs is not None else {}),
                        **({"e2e_path": "HostPipelinedLinear: 4 slabs of M, H2D / GEMM / D2H on three streams"}
                           if pipe is not None else {})},
             "roofline": {"bound": wl["bound"], "achieved": achieved, "peak": peak, "unit": unit,
-                         "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src, "kernel_ms": ms_kernel},
+                         "frac": achieved / peak, "peak_source": peak_src, "kernel_ms": ms_kernel},
             "e2e": {"value": scale_f(ms_e2e), "unit": unit, "h2d_bytes_per_step": x_host.numel() * x_host.element_size(),
                     "d2h_bytes_per_step": y_host.numel() * y_host.element_size(), "ms_per_step": ms_e2e},
             "gpu_launches": steps * (1 if (world == 1 or fg is not None) else 2),
@@ -750,6 +752,8 @@ class Bench:
             y_host.copy_(out_g, non_blocking=True)
 
         ms_dev = self.timed(lambda i: graph.replay(), args.steps, self.warm)
+        if name == args.workload and args.dump_outputs:
+            self.dump_output(out_g)  # the graph's output buffer holds the last timed step's result
         ms_e2e = self.timed(e2e_step, args.steps, self.warm)
         self.load_for_clocks(lambda i: graph.replay(), mark, max_seconds=1.0)
         clocks = self.sampler.snapshot(mark)
@@ -763,7 +767,7 @@ class Bench:
                        "l2": "3.7 GB of weights per step >> L2", "launch": "one CUDA graph per step",
                        "note": "quantized linears only (lm_head, attention, norms excluded)"},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": self.peaks["hbm"], "unit": "GB/s",
-                         "frac": achieved / self.peaks["hbm"], "traffic": None, "peak_source": self.peaks["source"],
+                         "frac": achieved / self.peaks["hbm"], "peak_source": self.peaks["source"],
                          "per_gpu": True},
             "e2e": {"value": M / (ms_e2e * 1e-3), "unit": "tokens/s", "h2d_bytes_per_step": x_host.numel() * 2,
                     "d2h_bytes_per_step": y_host.numel() * 2, "ms_per_step": ms_e2e},
@@ -777,9 +781,9 @@ class Bench:
 
     # ---- the kernels the reference would dispatch to on this GPU, same shapes, same process ---------------------------
     def compare_set(self):
-        """SURVEY 2.2 / BASELINE.md 5: what optimum-quanto itself runs on a B200 for these layers -- library kernels, timed
+        """SURVEY 2.2 / BASELINE.md 5: what optimum-quanto itself runs on this GPU for these layers -- library kernels, timed
         here so that the comparison is same-box, same-run.  (The reference's own AWQ / Marlin CUDA sources JIT-compile
-        only from its package; tools/compare_reference_kernels.py times them when oracle/_ref carries it.)"""
+        only from its package.)"""
         dev = self.dev
         out = {}
         M, N, K = 4096, N_DIM, K_DIM
@@ -840,6 +844,19 @@ class Bench:
         torch.cuda.empty_cache()
         return out
 
+    def dump_output(self, y):
+        """--dump-outputs DIR: the [M, N] output a caller of the timed path receives, as float32 `out.npy`; above
+        DUMP_ROWS rows, the rows of a fixed seeded sample (sorted), so that two builds can be compared output for output."""
+        if self.rank != 0:
+            return
+        import numpy as np
+        rows = np.arange(y.shape[0])
+        if y.shape[0] > DUMP_ROWS:
+            rows = np.sort(np.random.default_rng(0).choice(y.shape[0], size=DUMP_ROWS, replace=False))
+        out = y[torch.from_numpy(rows).to(y.device)].float().cpu().numpy()
+        os.makedirs(self.args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(self.args.dump_outputs, "out.npy"), out)
+
     # ---- top level --------------------------------------------------------------------------------------------------
     def run(self):
         args = self.args
@@ -893,7 +910,11 @@ def main():
     ap.add_argument("--gather", default="fused", choices=["fused", "nccl"],
                     help="multi-GPU int4: all-gather fused into the kernel (default) or kernel + NCCL all-gather")
     ap.add_argument("--no-extras", action="store_true", help="default workload only: skip the extra / compare sections")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the output of the last timed step of the --workload to DIR/out.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs dumps the outputs of --impl ours")
     wl = WORKLOADS[args.workload]
     if args.impl == "reference":
         if wl["kind"] == "llama":

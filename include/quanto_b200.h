@@ -1,4 +1,4 @@
-/* quanto_b200 -- C ABI of the B200-native quantized-linear hot path.
+/* quanto_b200 -- C ABI of the H100-native quantized-linear hot path.
  *
  * This is the drop-in boundary for the CUDA side of huggingface/optimum-quanto's quantized linear forward
  * (reference commit e33f8202).  Every entry point takes raw DEVICE pointers and sizes, enqueues work on the
@@ -31,7 +31,7 @@ extern "C" {
 #define QB200_ERR_ARG 1         /* bad problem description (shape, dtype, alignment)  ~ ERR_PROB_SHAPE */
 #define QB200_ERR_UNSUPPORTED 2 /* no kernel for this configuration                  ~ ERR_KERN_SHAPE */
 #define QB200_ERR_CUDA 3        /* a CUDA runtime / driver call failed (see qb200_last_error) */
-#define QB200_ERR_ARCH 4        /* device is not sm_100 */
+#define QB200_ERR_ARCH 4        /* device is not sm_90 */
 
 /* element types */
 #define QB200_F32 0
@@ -81,11 +81,12 @@ QB200_API int qb200_dequantize_qbits(const uint8_t* packed, const void* scale, c
  * shift_is_int), group divides K (per-axis quantisation: group = K).  dtype in {F32, F16, BF16} (A, scale, shift, bias,
  * out); bits in {2, 4}.
  * Kernel selection: 4-bit, F16 / BF16, N even, K % 16 == 0, group 32 or a multiple of 64 and 16-byte aligned buffers run
- * on the tcgen05 / TMA kernels (M <= 8: TMA-ring gemv; M <= 128: stream-K kernels; larger M: persistent GEMM); every
+ * on the TMA / tensor-core kernels (M <= 16: TMA-ring gemvs; M <= 8 shapes they decline: stream-K gemv; otherwise the
+ * persistent wgmma GEMM); every
  * other valid problem runs on a shape-agnostic CUDA-core kernel with the same operands and rounding order -- there is
  * no library / eager fallback behind this entry point.
  *
- * `workspace` (device memory, may be NULL): scratch for the small-M stream-K kernels, at least
+ * `workspace` (device memory, may be NULL): scratch for the small-M stream-K gemv, at least
  * qb200_qbits_mm_workspace_bytes(m, n, k) bytes, ZERO-INITIALISED ONCE by the caller (the kernel leaves its ticket
  * counters zero on exit) and not shared between streams that run concurrently.  Like the caller-provided zeroed
  * `workspace` of the reference's marlin binding (optimum/quanto/tensor/weights/marlin/int4/qbits.py:101).  Without
@@ -190,31 +191,28 @@ QB200_API int qb200_quantize_qbytes_absmax(const void* base, void* out, void* sc
                                            int out_dtype, void* stream);
 
 /* Which kernel family the last qb200_qbytes_mm / qb200_qbits_mm call on this thread dispatched to:
- * 0 none, 1 tcgen05 (TMA + TMEM), 2 CUDA-core (shape-agnostic), 3 warp-MMA gemv (int4, M <= 32: TMA ring or register streaming).
+ * 0 none, 1 wgmma (TMA + warpgroup MMA), 2 CUDA-core (shape-agnostic), 3 warp-MMA gemv (int4, M <= 32: TMA ring or register streaming).
  * For tests and bench accounting. */
 QB200_API int qb200_last_kernel_family(void);
 
 /* Test hook: choose among kernels that all compute the same result, so that a test-suite can execute every shipped
  * instantiation (value 0 = automatic choice, the default).  Process-wide.
- *   key 0  int4 large-M tile width        : 224 | 256
- *   key 1  int8 / fp8 pair-kernel tile N   : 224 | 256
- *   key 2  int4 route                      : 1 general tcgen05 kernel, 2 tcgen05 decode kernel (M <= 128),
- *                                            3 warp-MMA gemv (M <= 32), 4 TMA-ring gemv (M <= 8), 5 CTA-pair kernel,
- *                                            6 CTA-pair kernel with the weight operand in tensor memory,
+ *   key 0  wgmma tile rows                 : 64 (one consumer warpgroup) | 128 (two)
+ *   key 1  int8 x int8 tile N              : 128 | 256
+ *   key 2  int4 route                      : 1 wgmma kernel, 3 warp-MMA gemv (M <= 32), 4 TMA-ring gemv (M <= 8),
  *                                            8 second-generation TMA-ring gemv (M <= 16)
- *   key 3  qbytes route                    : 1 one CTA per tile (no pairs), 2 CUDA-core kernel
- *   key 4  int4 epilogue                   : 1 per-lane stores, 2 staged TMA stores
- *   key 5  ring-gemv producer              : 1 one issuing thread, 2 one lane per packed row, 3 32 lanes
- *   key 6  programmatic dependent launch   : 1 off
- *   key 7  ring-gemv shape (M <= 2)        : 2 two CTAs per SM (opt-in experiment; default one CTA per SM) */
+ *   key 3  qbytes route                    : 2 CUDA-core kernel
+ *   key 4  ring-gemv producer              : 1 one issuing thread, 2 one lane per packed row, 3 32 lanes
+ *   key 5  programmatic dependent launch   : 1 off
+ *   key 6  ring-gemv shape (M <= 2)        : 2 two CTAs per SM (opt-in experiment; default one CTA per SM) */
 QB200_API int qb200_test_override(int key, int value);
 
 /* Developer aids.  They act only in a library built with `make KNOCKOUTS=1` (qb200_developer_build() == 1); in the
  * release library the setters are no-ops and qb200_debug_flags() is always 0.
- *   qb200_debug_set_trace : device buffer of >= 4*5*64 int64 for clock64 stamps of the pipeline roles (tools/trace_*.py)
+ *   qb200_debug_set_trace : device buffer of >= 4*5*64 int64 for clock64 stamps of the pipeline roles
  *   qb200_debug_set_flags : timing knock-outs, results are WRONG while set: 1 skip dequant arithmetic, 2 skip the MMA,
  *                           4 constant scales, 8 skip activations / stream only, 16 no segment end,
- *                           64 skip the pair kernel's epilogue, 128 L2-hot operand loads, 256 no output rows,
+ *                           256 no output rows,
  *                           512 extra trace stamps */
 QB200_API void qb200_debug_set_trace(void* device_buffer);
 QB200_API void qb200_debug_set_flags(int flags);

@@ -82,14 +82,14 @@ static DeviceFacts g_dev[kMaxDevices];
 
 int current_sm_count() {
   const int dev = current_device();
-  if (dev < 0) return kNumSMsB200;
+  if (dev < 0) return kNumSMsH100;
   if (dev < kMaxDevices) {
     const int cached = g_dev[dev].sms.load(std::memory_order_relaxed);
     if (cached > 0) return cached;
   }
   int sms = 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (sms <= 0) sms = kNumSMsB200;
+  if (sms <= 0) sms = kNumSMsH100;
   if (dev < kMaxDevices) g_dev[dev].sms.store(sms, std::memory_order_relaxed);
   return sms;
 }
@@ -103,7 +103,7 @@ int check_arch() {
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
     if (dev < kMaxDevices) g_dev[dev].cc_major.store(major, std::memory_order_relaxed);
   }
-  return major == 10 ? OK : fail(ERR_ARCH, "quanto_b200 kernels are built for sm_100a only (device %d is sm_%d)", dev, major);
+  return major == 9 ? OK : fail(ERR_ARCH, "quanto_b200 kernels are built for sm_90a only (device %d is sm_%d)", dev, major);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -173,7 +173,7 @@ int qb200_version(void) { return 200; }
 int qb200_device_supported(int device) {
   int major = 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device) != cudaSuccess) return -1;
-  return major == 10 ? 1 : 0;
+  return major == 9 ? 1 : 0;
 }
 
 const char* qb200_last_error(void) { return g_err; }

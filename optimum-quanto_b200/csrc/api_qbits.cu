@@ -1,12 +1,11 @@
-// qb200_qbits_mm / qb200_qbits_mm_gather: argument checks, kernel selection and the large-M tcgen05 instantiations of the
-// fused packed-int4 linear (gemm_tc.cuh, gemm_tc2.cuh).  The small-M kernels live in api_qbits_small.cu.
+// qb200_qbits_mm / qb200_qbits_mm_gather: argument checks, kernel selection and the wgmma instantiations of the fused
+// packed-int4 linear (gemm_tc.cuh).  The small-M gemv kernels live in api_qbits_small.cu.
 #include "../../include/quanto_b200.h"
 
 #include <cstring>
 
 #include "api_qbits.cuh"
 #include "gemm_tc.cuh"
-#include "gemm_tc2.cuh"
 
 namespace qb {
 
@@ -14,39 +13,26 @@ int launch_qbits_mm_simt(const void*, const uint8_t*, const void*, const void*, 
                          int, int, int, int64_t, int64_t, cudaStream_t);
 
 template <class Cfg>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const StoreMaps& sm, const GemmParams& p,
-                       uint32_t idesc, cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap& ta, const GemmParams& p, cudaStream_t stream) {
   int rc = ensure_dyn_smem<gemm_tc_kernel<Cfg>>(Cfg::SMEM_BYTES);
   if (rc != OK) return rc;
+  CUtensorMap tb;
+  std::memset(&tb, 0, sizeof(tb));  // the weight tile is staged by the kernel's own warps
   const int tiles = p.num_m_blocks * p.num_n_blocks;
   const int grid = tiles < current_sm_count() ? tiles : current_sm_count();
-  gemm_tc_kernel<Cfg><<<grid, Cfg::NTHREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, sm, p, idesc);
+  gemm_tc_kernel<Cfg><<<grid, Cfg::NTHREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, p);
   return check_cuda(cudaGetLastError(), "gemm_tc_kernel launch");
 }
 
-template <class Cfg>
-static int launch_gemm_pair(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, uint32_t idesc,
-                            cudaStream_t stream) {
-  int rc = ensure_dyn_smem<gemm_tc2_kernel<Cfg>>(Cfg::SMEM_BYTES);
-  if (rc != OK) return rc;
-  const int tiles = p.num_m_blocks * p.num_n_blocks;
-  const int pairs = current_sm_count() / 2;
-  const int grid = 2 * (tiles < pairs ? tiles : pairs);
-  gemm_tc2_kernel<Cfg><<<grid, Cfg::NTHREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, p, idesc);
-  return check_cuda(cudaGetLastError(), "gemm_tc2_kernel launch");
-}
-
-template <int MS, int BNV, int EPI>
-static int launch_int4(const CUtensorMap& ta, const CUtensorMap& tb, const StoreMaps& sm, const GemmParams& p, int dtype,
-                       bool zp, cudaStream_t st) {
-  const uint32_t fmt = (dtype == DT_BF16) ? 1u : 0u;
-  const uint32_t idesc = umma_idesc(1u, fmt, fmt, 128u, BNV);
+template <int MWG>
+static int launch_int4(const CUtensorMap& ta, const GemmParams& p, int dtype, bool zp, cudaStream_t st) {
+  constexpr int BN = 128;
   if (dtype == DT_BF16) {
-    if (zp) return launch_gemm<GemmCfg<MmaKind::F16, BSrc::INT4, MS, BNV, __nv_bfloat16, true, 0, EPI>>(ta, tb, sm, p, idesc, st);
-    return launch_gemm<GemmCfg<MmaKind::F16, BSrc::INT4, MS, BNV, __nv_bfloat16, false, 0, EPI>>(ta, tb, sm, p, idesc, st);
+    if (zp) return launch_gemm<GemmCfg<MmaKind::BF16, BSrc::INT4, MWG, BN, __nv_bfloat16, true>>(ta, p, st);
+    return launch_gemm<GemmCfg<MmaKind::BF16, BSrc::INT4, MWG, BN, __nv_bfloat16, false>>(ta, p, st);
   }
-  if (zp) return launch_gemm<GemmCfg<MmaKind::F16, BSrc::INT4, MS, BNV, __half, true, 0, EPI>>(ta, tb, sm, p, idesc, st);
-  return launch_gemm<GemmCfg<MmaKind::F16, BSrc::INT4, MS, BNV, __half, false, 0, EPI>>(ta, tb, sm, p, idesc, st);
+  if (zp) return launch_gemm<GemmCfg<MmaKind::F16, BSrc::INT4, MWG, BN, __half, true>>(ta, p, st);
+  return launch_gemm<GemmCfg<MmaKind::F16, BSrc::INT4, MWG, BN, __half, false>>(ta, p, st);
 }
 
 static int qbits_mm_impl(QbitsArgs& q) {
@@ -62,7 +48,6 @@ static int qbits_mm_impl(QbitsArgs& q) {
   int rc = check_arch();
   if (rc != OK) return rc;
   const bool gathered = q.g.n_out > 1;
-  const bool plain_out = !gathered && q.ld == n && q.col0 == 0;
   // tensor-core kernels: 4-bit, 16-bit activations, N even, K % 16 == 0, group 32 or a multiple of 64, aligned buffers.
   // Everything else runs on the shape-agnostic CUDA-core kernel (same operands, same rounding order).
   const bool tc_ok = q.bits == 4 && (dtype == DT_BF16 || dtype == DT_F16) && n % 2 == 0 && k % 16 == 0 &&
@@ -83,7 +68,6 @@ static int qbits_mm_impl(QbitsArgs& q) {
   rc = qbits_small_dispatch(q, &handled);
   if (rc != OK || handled) return rc;
 
-  cudaStream_t st = q.stream;
   GemmParams p{};
   p.scales = nullptr;
   p.bias = q.bias;
@@ -101,70 +85,20 @@ static int qbits_mm_impl(QbitsArgs& q) {
   p.group = group;
   p.group_log2 = q.group_log2;
   p.shift_is_int = q.shift_is_int;
-  p.trace = debug_trace();
-  p.dbg = debug_flags();
-  CUtensorMap ta, tb;
-  StoreMaps sm;
-  std::memset(&tb, 0, sizeof(tb));
-  std::memset(&sm, 0, sizeof(sm));
-  rc = make_tmap_2d(&ta, q.a, dtype, m, k, 128);
+  // Tile M: one consumer warpgroup (64 rows) while M <= 64, so that small batches do not pay for empty MMA rows.
+  int tile_m = m <= 64 ? 64 : 128;
+  const int force_m = test_override(OVR_TILE_M);
+  if (force_m == 64 || force_m == 128) tile_m = force_m;
+  constexpr int BN = 128;  // out-features per tile: 64 packed rows, both nibble planes
+  p.num_m_blocks = static_cast<int>((m + tile_m - 1) / tile_m);
+  p.num_n_blocks = static_cast<int>((n / 2 + BN / 2 - 1) / (BN / 2));
+  CUtensorMap ta;
+  rc = make_tmap_2d(&ta, q.a, dtype, m, k, tile_m);
   if (rc != OK) return rc;
   set_kernel_family(1);
   const bool zp = q.shift_is_int != 0;
-  const int sms = current_sm_count();
-  const bool big = m > 128;
-  auto n_blocks = [&](int bn) { return static_cast<int>((n / 2 + bn / 2 - 1) / (bn / 2)); };
-  const int route = test_override(OVR_INT4_ROUTE);
-
-  if (big && route == ROUTE_INT4_PAIR && plain_out) {
-    // CTA pairs (cta_group::2): 256 x 256 tile per pair, each CTA dequantises the packed rows of its half of the
-    // out-features only.  Measured no faster than the single-CTA kernel (the A operand is not multicast): test hook only.
-    constexpr int BNP = 256;
-    p.num_m_blocks = static_cast<int>((m + 255) / 256);
-    p.num_n_blocks = n_blocks(BNP);
-    const uint32_t fmt = (dtype == DT_BF16) ? 1u : 0u;
-    const uint32_t idesc = umma_idesc(1u, fmt, fmt, 256u, BNP);
-    if (dtype == DT_BF16) {
-      if (zp) return launch_gemm_pair<PairCfg<MmaKind::F16, BNP, BSrc::INT4, __nv_bfloat16, true>>(ta, tb, p, idesc, st);
-      return launch_gemm_pair<PairCfg<MmaKind::F16, BNP, BSrc::INT4, __nv_bfloat16, false>>(ta, tb, p, idesc, st);
-    }
-    if (zp) return launch_gemm_pair<PairCfg<MmaKind::F16, BNP, BSrc::INT4, __half, true>>(ta, tb, p, idesc, st);
-    return launch_gemm_pair<PairCfg<MmaKind::F16, BNP, BSrc::INT4, __half, false>>(ta, tb, p, idesc, st);
-  }
-
-  // ---- epilogue: the staged TMA-store form needs whole 64-column blocks per nibble half and 16-byte aligned rows
-  const bool tma_store_ok = ((n / 2) % 64 == 0) && ((q.ld * 2) % 16 == 0) && ((q.col0 * 2) % 16 == 0);
-  // ---- M > 128: CTA pairs with the weight operand in tensor memory (gemm_w4p.cuh) when the problem fits its tiling
-  const bool w4p_ok = big && tma_store_ok && k % 128 == 0 && (group == 32 || group == 64 || group % 128 == 0);
-  if (w4p_ok && (route == ROUTE_INT4_PAIR_TMEM || (route == ROUTE_AUTO && kW4PDefault))) return launch_w4p(q);
-  if (route == ROUTE_INT4_PAIR_TMEM) return fail(ERR_UNSUPPORTED, "qbits_mm: the TMEM pair kernel needs M > 128, K %% 128 == 0, (N / 2) %% 64 == 0");
-  if (!plain_out && !tma_store_ok)
-    return fail(ERR_UNSUPPORTED, "qbits_mm_gather: needs (n_local / 2) %% 64 == 0 and 16-byte aligned output rows");
-  p.num_m_blocks = big ? static_cast<int>((m + 255) / 256) : 1;
-  // Tile N: 256, or 224 when that fills the last wave better (e.g. N = 14336: 896 tiles = 6.05 waves of 148 CTAs
-  // with 256, 1024 tiles = 6.92 waves with 224).  Cost model: rounds x per-tile MMA time (proportional to N).
-  auto cost = [&](int bn) {
-    const long tiles = static_cast<long>(p.num_m_blocks) * n_blocks(bn);
-    return ((tiles + sms - 1) / sms) * bn;
-  };
-  int bn = (big && cost(224) < cost(256)) ? 224 : 256;
-  const int force_bn = test_override(OVR_INT4_TILE_N);
-  if (force_bn == 224 || force_bn == 256) bn = force_bn;
-  if (!plain_out) bn = 256;
-  int epi = (bn == 256 && tma_store_ok) ? 1 : 0;
-  const int force_epi = test_override(OVR_EPILOGUE);
-  if (plain_out && force_epi == 1) epi = 0;
-  if (force_epi == 2 && tma_store_ok) { epi = 1; bn = 256; }
-  p.num_n_blocks = n_blocks(bn);
-  if (epi == 1) {
-    for (int i = 0; i < q.g.n_out; ++i) {
-      rc = make_tmap_2d_view(&sm.m[i], q.g.out_peer[i], dtype, m, q.ld, q.ld, 64, 32, true);
-      if (rc != OK) return rc;
-    }
-    return big ? launch_int4<2, 256, 1>(ta, tb, sm, p, dtype, zp, st) : launch_int4<1, 256, 1>(ta, tb, sm, p, dtype, zp, st);
-  }
-  if (bn == 224) return big ? launch_int4<2, 224, 0>(ta, tb, sm, p, dtype, zp, st) : launch_int4<1, 224, 0>(ta, tb, sm, p, dtype, zp, st);
-  return big ? launch_int4<2, 256, 0>(ta, tb, sm, p, dtype, zp, st) : launch_int4<1, 256, 0>(ta, tb, sm, p, dtype, zp, st);
+  if (tile_m == 64) return launch_int4<1>(ta, p, dtype, zp, q.stream);
+  return launch_int4<2>(ta, p, dtype, zp, q.stream);
 }
 
 }  // namespace qb

@@ -1,5 +1,5 @@
-// Shared between the translation units of the fused packed-int4 linear (api_qbits.cu: dispatcher + large-M kernels,
-// api_qbits_small.cu: decode kernels).
+// Shared between the translation units of the fused packed-int4 linear (api_qbits.cu: dispatcher + wgmma kernel,
+// api_qbits_small.cu: gemv kernels).
 #pragma once
 
 #include "gather.cuh"
@@ -28,10 +28,4 @@ int64_t qbits_small_workspace_bytes(int64_t m, int64_t n, int64_t k);
 int qbits_ring_plan(int64_t m, int64_t n, int64_t k, int group, int zp, int grid, int* out);
 int qbits_small_dispatch(const QbitsArgs& q, bool* handled);
 
-}  // namespace qb
-
-namespace qb {
-// M > 128: CTA-pair kernel with the weight operand in tensor memory (gemm_w4p.cuh, api_qbits_w4p.cu)
-constexpr bool kW4PDefault = true;  // measured (tools/gemv_modes.py): 1.10-1.5x the single-CTA kernel on every Llama shape
-int launch_w4p(const QbitsArgs& q);
 }  // namespace qb

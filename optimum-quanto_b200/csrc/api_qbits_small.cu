@@ -1,7 +1,6 @@
-// Small-M ("decode") launchers of the fused packed-int4 linear: the TMA-ring gemv (M <= 8), the register-streaming
-// warp-MMA kernel (M <= 32) and the tcgen05 kernel with the weight operand in tensor memory (M <= 128).
+// Small-M ("decode") launchers of the fused packed-int4 linear: the TMA-ring gemvs (M <= 16) and the
+// register-streaming warp-MMA kernel (M <= 32).  Everything else goes to the wgmma kernel (api_qbits.cu).
 #include "api_qbits.cuh"
-#include "gemm_decode.cuh"
 #include "gemv_w4.cuh"
 #include "gemv_w4s.cuh"
 #include "gemv_w4r.cuh"
@@ -19,16 +18,16 @@ static bool decode_applicable(int64_t m, int64_t n, int64_t k) {
   return m >= 1 && m <= 128 && n % 2 == 0 && k % 128 == 0 && (n / 2 + 63) / 64 <= kDecodeTicketBytes / 4;
 }
 
-// M <= kGemvMaxM: register-streaming warp-MMA kernel (gemv_w4.cuh), several CTAs per SM;
-// kGemvMaxM < M <= 128: tcgen05 kernel with the A operand in tensor memory (gemm_decode.cuh), one CTA per SM.
-constexpr int kGemvMaxM = 8;   // measured (tools/gemv_modes.py): for 8 < M <= 32 the tcgen05 kernel is 1.3-2x faster
+// M <= kGemvMaxM (shapes the ring gemvs do not take): register-streaming warp-MMA kernel (gemv_w4.cuh), several CTAs
+// per SM; larger M goes to the wgmma kernel.
+constexpr int kGemvMaxM = 8;
 
-static DecodePlan make_decode_plan(int64_t m, int64_t n, int64_t k, int sms, bool gemv) {
+static DecodePlan make_decode_plan(int64_t m, int64_t n, int64_t k, int sms) {
   DecodePlan pl;
   pl.P = static_cast<int>((n / 2 + 63) / 64);
   pl.SPB = static_cast<int>(k / 128);  // 128-k stages per out-feature block
   const int total = pl.P * pl.SPB;
-  const int ctas_per_sm = !gemv ? 1 : (m <= 16 ? 3 : 2);
+  const int ctas_per_sm = m <= 16 ? 3 : 2;
   const int slots = sms * ctas_per_sm;
   int grid = total < slots ? total : slots;
   pl.span = (total + grid - 1) / grid;
@@ -43,21 +42,9 @@ static DecodePlan make_decode_plan(int64_t m, int64_t n, int64_t k, int sms, boo
 
 int64_t qbits_small_workspace_bytes(int64_t m, int64_t n, int64_t k) {
   if (!decode_applicable(m, n, k)) return 0;
-  // sized for the worst case over both kernels and SM counts up to the B200's 148 (the plan is made per device at call time)
-  DecodePlan a = make_decode_plan(m, n, k, kNumSMsB200, true), b = make_decode_plan(m, n, k, kNumSMsB200, false);
-  const int64_t pa = a.partial_bytes > b.partial_bytes ? a.partial_bytes : b.partial_bytes;
-  return a.ticket_bytes + pa;
-}
-
-template <class Cfg>
-static int launch_decode(const CUtensorMap& tw, const CUtensorMap& tx, const DecodeParams& p, uint32_t idesc, int grid,
-                         cudaStream_t stream) {
-  int rc = ensure_dyn_smem<gemm_w4_decode_kernel<Cfg>>(Cfg::SMEM_BYTES);
-  if (rc != OK) return rc;
-  const bool pdl = test_override(OVR_PDL) != 1;
-  return check_cuda(launch_kernel_pdl(gemm_w4_decode_kernel<Cfg>, dim3(grid), dim3(Cfg::NTHREADS), Cfg::SMEM_BYTES, stream,
-                                      pdl, tw, tx, p, idesc),
-                    "gemm_w4_decode_kernel launch");
+  // sized for the H100's 132 SMs (the plan is made per device at call time and checked against the size)
+  const DecodePlan a = make_decode_plan(m, n, k, kNumSMsH100);
+  return a.ticket_bytes + a.partial_bytes;
 }
 
 template <typename WT, int MT, bool ZP>
@@ -135,18 +122,6 @@ static int launch_gemvs(const GemvSParams& p, int grid, int smem_bytes, cudaStre
   return launch_gemvs_cr<WT, ZP, false, 0>(p, grid, smem_bytes, stream);
 }
 
-template <typename WT, bool ZP>
-static int launch_decode_mp(int mp, const CUtensorMap& tw, const CUtensorMap& tx, const DecodeParams& p, uint32_t fmt,
-                            int grid, cudaStream_t stream) {
-  const uint32_t idesc = umma_idesc(1u, fmt, fmt, 128u, static_cast<uint32_t>(mp));
-  switch (mp) {
-    case 16: return launch_decode<DecodeCfg<WT, 16, ZP>>(tw, tx, p, idesc, grid, stream);
-    case 32: return launch_decode<DecodeCfg<WT, 32, ZP>>(tw, tx, p, idesc, grid, stream);
-    case 64: return launch_decode<DecodeCfg<WT, 64, ZP>>(tw, tx, p, idesc, grid, stream);
-    default: return launch_decode<DecodeCfg<WT, 128, ZP>>(tw, tx, p, idesc, grid, stream);
-  }
-}
-
 // ---------------------------------------------------------------------------------------------
 // M <= 16, group 64 / 128, K % 1024 == 0: second-generation TMA-ring gemv (gemv_w4r.cuh), compile-time shaped loop
 // ---------------------------------------------------------------------------------------------
@@ -215,8 +190,8 @@ static bool make_gemvr_plan(int64_t m, int64_t n, int64_t k, int group, bool zp,
     const int64_t stage = 8 * (kc + 64);
     for (int nxc = 1; nxc <= nk; ++nxc) {
       if (nk % nxc != 0) continue;
-      // several passes cost a pipeline drain each: worth it for M <= 8, where this kernel is the only one whose k-order
-      // does not depend on the shard (measured at M = 16, K = 14336: 40 us against 31 us for the tcgen05 decode kernel)
+      // several passes cost a pipeline drain each: worth it for M <= 8 only, where this kernel is the only one whose
+      // k-order does not depend on the shard
       if (nxc > 1 && m > 8) break;
       const int nkc = nk / nxc;
       const int64_t kx = k / nxc;
@@ -315,7 +290,7 @@ int qbits_small_dispatch(const QbitsArgs& q, bool* handled) {
   *handled = false;
   const int64_t m = q.m, n = q.n, k = q.k;
   const int route = test_override(OVR_INT4_ROUTE);
-  if (route == ROUTE_INT4_GENERAL || route == ROUTE_INT4_PAIR || route == ROUTE_INT4_PAIR_TMEM || route == ROUTE_INT4_SINGLE) return OK;
+  if (route == ROUTE_INT4_GENERAL) return OK;
   cudaStream_t st = q.stream;
   const bool bf16 = q.dtype == DT_BF16;
   const bool zp = q.shift_is_int != 0;
@@ -399,25 +374,17 @@ int qbits_small_dispatch(const QbitsArgs& q, bool* handled) {
     if (route == ROUTE_INT4_RING) return fail(ERR_UNSUPPORTED, "qbits_mm: the ring gemv does not take this problem");
   }
 
-  if (!decode_applicable(m, n, k) || q.workspace == nullptr) {
-    if (route != ROUTE_AUTO) return fail(ERR_UNSUPPORTED, "qbits_mm: the requested small-M kernel needs M <= 128, K %% 128 == 0 and a workspace");
+  // register-streaming gemv: M <= 8 (M <= 32 on request), one plain [M, N] output (no fused gather)
+  const bool want_gemv = route == ROUTE_INT4_GEMV || (route == ROUTE_AUTO && m <= kGemvMaxM);
+  if (!want_gemv) return OK;
+  if (route == ROUTE_INT4_GEMV && m > 32) return fail(ERR_UNSUPPORTED, "qbits_mm: the warp-MMA gemv takes M <= 32");
+  const bool gemv_ok = decode_applicable(m, n, k) && q.workspace != nullptr && q.g.n_out == 1 && q.ld == q.n &&
+                       q.col0 == 0 && q.group % 16 == 0 && reinterpret_cast<uintptr_t>(q.a) % 8 == 0;
+  DecodePlan pl = make_decode_plan(m, n, k, current_sm_count());
+  if (!gemv_ok || pl.ticket_bytes + pl.partial_bytes > q.workspace_bytes || reinterpret_cast<uintptr_t>(q.workspace) % 256 != 0) {
+    if (route != ROUTE_AUTO) return fail(ERR_UNSUPPORTED, "qbits_mm: the warp-MMA gemv needs K %% 128 == 0, a plain output and a large enough workspace");
     return OK;
   }
-  bool use_gemv = (m <= kGemvMaxM);
-  if (route == ROUTE_INT4_TCDECODE) use_gemv = false;
-  if (route == ROUTE_INT4_GEMV) {
-    if (m > 32) return fail(ERR_UNSUPPORTED, "qbits_mm: the warp-MMA gemv takes M <= 32");
-    use_gemv = true;
-  }
-  // the register-streaming gemv writes one plain [M, N] output (no fused gather)
-  if (use_gemv && (q.g.n_out > 1 || q.ld != q.n || q.col0 != 0)) use_gemv = false;
-  if (use_gemv && !(q.group % 16 == 0 && reinterpret_cast<uintptr_t>(q.a) % 8 == 0)) use_gemv = false;
-  DecodePlan pl = make_decode_plan(m, n, k, current_sm_count(), use_gemv);
-  if (pl.ticket_bytes + pl.partial_bytes > q.workspace_bytes || reinterpret_cast<uintptr_t>(q.workspace) % 256 != 0) {
-    if (route != ROUTE_AUTO) return fail(ERR_UNSUPPORTED, "qbits_mm: workspace too small or unaligned");
-    return OK;
-  }
-  const int mp = m <= 16 ? 16 : (m <= 32 ? 32 : (m <= 64 ? 64 : 128));
   DecodeParams d{};
   d.scale = q.scale;
   d.shift = q.shift;
@@ -438,32 +405,16 @@ int qbits_small_dispatch(const QbitsArgs& q, bool* handled) {
   d.SPB = pl.SPB;
   d.span = pl.span;
   d.max_segs = pl.max_segs;
-  d.trace = debug_trace();
   d.dbg = dbg;
   *handled = true;
-  if (use_gemv) {
-    set_kernel_family(3);
-    const int mi = static_cast<int>(m);
-    if (bf16) {
-      if (zp) return launch_gemv_mt<__nv_bfloat16, true>(mi, q.packed, q.a, d, pl.grid, st);
-      return launch_gemv_mt<__nv_bfloat16, false>(mi, q.packed, q.a, d, pl.grid, st);
-    }
-    if (zp) return launch_gemv_mt<__half, true>(mi, q.packed, q.a, d, pl.grid, st);
-    return launch_gemv_mt<__half, false>(mi, q.packed, q.a, d, pl.grid, st);
-  }
-  CUtensorMap tw, tx;
-  int rc = make_tmap_2d(&tw, q.packed, DT_U8, n / 2, k, 64);
-  if (rc != OK) return rc;
-  rc = make_tmap_2d(&tx, q.a, q.dtype, m, k, mp);
-  if (rc != OK) return rc;
-  set_kernel_family(1);
-  const uint32_t fmt = bf16 ? 1u : 0u;
+  set_kernel_family(3);
+  const int mi = static_cast<int>(m);
   if (bf16) {
-    if (zp) return launch_decode_mp<__nv_bfloat16, true>(mp, tw, tx, d, fmt, pl.grid, st);
-    return launch_decode_mp<__nv_bfloat16, false>(mp, tw, tx, d, fmt, pl.grid, st);
+    if (zp) return launch_gemv_mt<__nv_bfloat16, true>(mi, q.packed, q.a, d, pl.grid, st);
+    return launch_gemv_mt<__nv_bfloat16, false>(mi, q.packed, q.a, d, pl.grid, st);
   }
-  if (zp) return launch_decode_mp<__half, true>(mp, tw, tx, d, fmt, pl.grid, st);
-  return launch_decode_mp<__half, false>(mp, tw, tx, d, fmt, pl.grid, st);
+  if (zp) return launch_gemv_mt<__half, true>(mi, q.packed, q.a, d, pl.grid, st);
+  return launch_gemv_mt<__half, false>(mi, q.packed, q.a, d, pl.grid, st);
 }
 
 }  // namespace qb

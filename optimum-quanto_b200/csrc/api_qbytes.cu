@@ -1,12 +1,11 @@
 // qb200_qbytes_mm / qb200_qbytes_mm_quantized: argument checks, kernel selection and the instantiations of the 8-bit
-// paths: int8 x int8 and fp8 x fp8 on tcgen05 (CTA pairs, gemm_tc2.cuh; one CTA per tile for M <= 128, gemm_tc.cuh),
-// weight-only fp16 / bf16 x int8 / fp8 with the conversion in the staging warps, and the shape-agnostic CUDA-core kernel.
+// paths: int8 x int8 on wgmma with both operands fed by TMA (gemm_tc.cuh), fp8 x fp8 and weight-only fp16 / bf16 x
+// int8 / fp8 with the conversion to 16 bits in the staging warps, and the shape-agnostic CUDA-core kernel.
 #include "../../include/quanto_b200.h"
 
 #include <cstring>
 
 #include "gemm_tc.cuh"
-#include "gemm_tc2.cuh"
 #include "host_common.cuh"
 
 namespace qb {
@@ -15,38 +14,39 @@ int launch_qbytes_mm_simt(const void*, const void*, const void*, const void*, vo
                           cudaStream_t);
 
 template <class Cfg>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, uint32_t idesc,
-                       cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
   int rc = ensure_dyn_smem<gemm_tc_kernel<Cfg>>(Cfg::SMEM_BYTES);
   if (rc != OK) return rc;
   const int tiles = p.num_m_blocks * p.num_n_blocks;
   const int grid = tiles < current_sm_count() ? tiles : current_sm_count();
-  static const StoreMaps no_maps{};  // these instantiations store from registers (GemmCfg::EPI == 0)
-  gemm_tc_kernel<Cfg><<<grid, Cfg::NTHREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, no_maps, p, idesc);
+  gemm_tc_kernel<Cfg><<<grid, Cfg::NTHREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, p);
   return check_cuda(cudaGetLastError(), "gemm_tc_kernel launch");
 }
 
-// CTA-pair kernel (gemm_tc2.cuh): clusters of 2 CTAs, one pair per 256 x BN tile.
-template <class Cfg>
-static int launch_gemm_pair(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, uint32_t idesc,
-                            cudaStream_t stream) {
-  int rc = ensure_dyn_smem<gemm_tc2_kernel<Cfg>>(Cfg::SMEM_BYTES);
-  if (rc != OK) return rc;
-  const int tiles = p.num_m_blocks * p.num_n_blocks;
-  const int pairs = current_sm_count() / 2;
-  const int grid = 2 * (tiles < pairs ? tiles : pairs);
-  gemm_tc2_kernel<Cfg><<<grid, Cfg::NTHREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, p, idesc);
-  return check_cuda(cudaGetLastError(), "gemm_tc2_kernel launch");
+// Columns of tensor-core work per SM for a tile of BM x bn: waves x bn (wave quantisation included).
+static int64_t wave_cost(int64_t m, int64_t n, int bm, int bn) {
+  const int64_t tiles = ((m + bm - 1) / bm) * ((n + bn - 1) / bn);
+  const int64_t sms = current_sm_count();
+  return ((tiles + sms - 1) / sms) * bn;
 }
 
-// Columns of tensor-core work per CTA pair for a pair tile of width bn: waves x bn (wave quantisation included).
-static int64_t pair_wave_cost(int64_t m, int64_t n, int bn) {
-  const int64_t tiles = ((m + 255) / 256) * ((n + bn - 1) / bn);
-  const int64_t pairs = current_sm_count() / 2;
-  return ((tiles + pairs - 1) / pairs) * bn;
+template <int MWG, int BN>
+static int launch_int8(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st) {
+  return launch_gemm<GemmCfg<MmaKind::I8, BSrc::TMA, MWG, BN>>(ta, tb, p, st);
 }
 
-static uint32_t fp8_fmt(int dt) { return dt == DT_E5M2 ? 1u : 0u; }
+// fp8 x fp8: both operands converted to bf16 by the staging warps (exact), bf16 MMAs with fp32 accumulation.  Hopper's
+// native fp8 MMA accumulates with fewer bits than fp32 and misses the exact-product / fp32-sum contract.
+template <int MWG>
+static int launch_fp8(int a_dt, int w_dt, const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p,
+                      cudaStream_t st) {
+  constexpr int BN = 128, E4 = 1, E5 = 2;
+  using BF = __nv_bfloat16;
+  if (a_dt == DT_E4M3 && w_dt == DT_E4M3) return launch_gemm<GemmCfg<MmaKind::BF16, BSrc::F8, MWG, BN, BF, false, E4, E4>>(ta, tb, p, st);
+  if (a_dt == DT_E4M3) return launch_gemm<GemmCfg<MmaKind::BF16, BSrc::F8, MWG, BN, BF, false, E5, E4>>(ta, tb, p, st);
+  if (w_dt == DT_E4M3) return launch_gemm<GemmCfg<MmaKind::BF16, BSrc::F8, MWG, BN, BF, false, E4, E5>>(ta, tb, p, st);
+  return launch_gemm<GemmCfg<MmaKind::BF16, BSrc::F8, MWG, BN, BF, false, E5, E5>>(ta, tb, p, st);
+}
 
 // q_dt != 0: the output is quantised in the epilogue (out = [M, N] bytes, q_scale = device pointer to the per-tensor
 // output scale in out_dtype); only the int8 x int8 / fp8 x fp8 tensor-core kernels do that.
@@ -80,10 +80,12 @@ static int qbytes_mm_impl(const void* a, const void* w, const void* scales, cons
     p.M = static_cast<int>(m);
     p.N = static_cast<int>(n);
     p.K = static_cast<int>(k);
-    p.trace = debug_trace();
-    p.dbg = debug_flags();
     return p;
   };
+  // Tile M: one consumer warpgroup (64 rows) while M <= 64, so that small batches do not pay for empty MMA rows.
+  int tile_m = m <= 64 ? 64 : 128;
+  const int force_m = test_override(OVR_TILE_M);
+  if (force_m == 64 || force_m == 128) tile_m = force_m;
 
   const bool both_i8 = (a_dtype == DT_I8 && w_dtype == DT_I8);
   const bool both_f8 = ((a_dtype == DT_E4M3 || a_dtype == DT_E5M2) && (w_dtype == DT_E4M3 || w_dtype == DT_E5M2));
@@ -94,38 +96,34 @@ static int qbytes_mm_impl(const void* a, const void* w, const void* scales, cons
     p.scales = scales;
     p.q_dt = q_dt;
     p.q_scale = q_scale;
+    // int8: tile N 128 or 256 (the wider tile reads A half as often), picked by wave cost; fp8: 128 (staged operands)
+    int bn = 128;
+    if (both_i8) {
+      bn = (tile_m == 128 && wave_cost(m, n, tile_m, 256) <= wave_cost(m, n, tile_m, 128)) ? 256 : 128;
+      const int force_bn = test_override(OVR_QBYTES_TILE_N);
+      if (force_bn == 128 || force_bn == 256) bn = force_bn;
+    }
+    p.num_m_blocks = static_cast<int>((m + tile_m - 1) / tile_m);
+    p.num_n_blocks = static_cast<int>((n + bn - 1) / bn);
     CUtensorMap ta, tb;
-    rc = make_tmap_2d(&ta, a, DT_U8, m, k, 128);
+    std::memset(&ta, 0, sizeof(ta));
+    std::memset(&tb, 0, sizeof(tb));
+    if (both_f8) {
+      p.a = a;  // the staging warps read both operands
+      p.wq = static_cast<const uint8_t*>(w);
+      set_kernel_family(1);
+      if (tile_m == 64) return launch_fp8<1>(a_dtype, w_dtype, ta, tb, p, st);
+      return launch_fp8<2>(a_dtype, w_dtype, ta, tb, p, st);
+    }
+    rc = make_tmap_2d(&ta, a, DT_U8, m, k, tile_m);
+    if (rc != OK) return rc;
+    rc = make_tmap_2d(&tb, w, DT_U8, n, k, bn);
     if (rc != OK) return rc;
     set_kernel_family(1);
-    const uint32_t dfmt = both_i8 ? 2u : 1u;
-    const uint32_t afmt = both_i8 ? 1u : fp8_fmt(a_dtype), bfmt = both_i8 ? 1u : fp8_fmt(w_dtype);
-    if (m > 128 && route != ROUTE_QBYTES_SINGLE) {
-      // CTA pairs (cta_group::2), 256 x BN tile per pair: 1.5x less L2 -> SM operand traffic per MAC than 128 x 256
-      // per CTA, which is what bounded the single-CTA kernel.  BN picked by wave cost.
-      int bn = pair_wave_cost(m, n, 224) < pair_wave_cost(m, n, 256) ? 224 : 256;
-      const int force_bn = test_override(OVR_QBYTES_TILE_N);
-      if (force_bn == 224 || force_bn == 256) bn = force_bn;
-      p.num_m_blocks = static_cast<int>((m + 255) / 256);
-      p.num_n_blocks = static_cast<int>((n + bn - 1) / bn);
-      rc = make_tmap_2d(&tb, w, DT_U8, n, k, bn / 2);
-      if (rc != OK) return rc;
-      const uint32_t idesc = umma_idesc(dfmt, afmt, bfmt, 256u, static_cast<uint32_t>(bn));
-      if (both_i8) {
-        if (bn == 224) return launch_gemm_pair<PairCfg<MmaKind::I8, 224>>(ta, tb, p, idesc, st);
-        return launch_gemm_pair<PairCfg<MmaKind::I8, 256>>(ta, tb, p, idesc, st);
-      }
-      if (bn == 224) return launch_gemm_pair<PairCfg<MmaKind::F8F6F4, 224>>(ta, tb, p, idesc, st);
-      return launch_gemm_pair<PairCfg<MmaKind::F8F6F4, 256>>(ta, tb, p, idesc, st);
+    {
+      if (tile_m == 64) return bn == 256 ? launch_int8<1, 256>(ta, tb, p, st) : launch_int8<1, 128>(ta, tb, p, st);
+      return bn == 256 ? launch_int8<2, 256>(ta, tb, p, st) : launch_int8<2, 128>(ta, tb, p, st);
     }
-    constexpr int BN = 256;
-    p.num_n_blocks = static_cast<int>((n + BN - 1) / BN);
-    p.num_m_blocks = static_cast<int>((m + 127) / 128);
-    rc = make_tmap_2d(&tb, w, DT_U8, n, k, BN);
-    if (rc != OK) return rc;
-    const uint32_t idesc = umma_idesc(dfmt, afmt, bfmt, 128u, BN);
-    if (both_i8) return launch_gemm<GemmCfg<MmaKind::I8, BSrc::TMA, 1, BN, __nv_bfloat16>>(ta, tb, p, idesc, st);
-    return launch_gemm<GemmCfg<MmaKind::F8F6F4, BSrc::TMA, 1, BN, __nv_bfloat16>>(ta, tb, p, idesc, st);
   }
   if (q_dt != 0)
     return fail(ERR_UNSUPPORTED, "qbytes_mm_quantized: needs int8 x int8 or fp8 x fp8 operands, K %% 16 == 0 and "
@@ -134,37 +132,33 @@ static int qbytes_mm_impl(const void* a, const void* w, const void* scales, cons
   const bool a_half = (a_dtype == DT_F16 || a_dtype == DT_BF16);
   if (a_half && out_dtype == a_dtype && (k % 16 == 0) && reinterpret_cast<uintptr_t>(a) % 16 == 0 &&
       reinterpret_cast<uintptr_t>(w) % 16 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0 && route != ROUTE_QBYTES_SIMT) {
-    constexpr int BN = 256;
+    constexpr int BN = 128;
     GemmParams p = base_params();
     p.scales = nullptr;  // applied to the weights before the MMA, like the reference does
     p.wq = static_cast<const uint8_t*>(w);
     p.wscale = scales;
     p.w_dt = w_dtype;
-    p.trace = nullptr;
     p.num_n_blocks = static_cast<int>((n + BN - 1) / BN);
-    const bool big = m > 128;
-    p.num_m_blocks = static_cast<int>(big ? (m + 255) / 256 : 1);
+    p.num_m_blocks = static_cast<int>((m + tile_m - 1) / tile_m);
     CUtensorMap ta, tb;
     std::memset(&tb, 0, sizeof(tb));
-    rc = make_tmap_2d(&ta, a, a_dtype, m, k, 128);
+    rc = make_tmap_2d(&ta, a, a_dtype, m, k, tile_m);
     if (rc != OK) return rc;
-    const uint32_t fmt = (a_dtype == DT_BF16) ? 1u : 0u;
-    const uint32_t idesc = umma_idesc(1u, fmt, fmt, 128u, BN);
     set_kernel_family(1);
-#define QB_LAUNCH_BYTES(WT, WK)                                                                                     \
-  (big ? launch_gemm<GemmCfg<MmaKind::F16, BSrc::BYTES, 2, BN, WT, false, WK>>(ta, tb, p, idesc, st)                 \
-       : launch_gemm<GemmCfg<MmaKind::F16, BSrc::BYTES, 1, BN, WT, false, WK>>(ta, tb, p, idesc, st))
+#define QB_LAUNCH_BYTES(KIND, WT, WK)                                                                   \
+  (tile_m == 128 ? launch_gemm<GemmCfg<KIND, BSrc::BYTES, 2, BN, WT, false, WK>>(ta, tb, p, st)         \
+                 : launch_gemm<GemmCfg<KIND, BSrc::BYTES, 1, BN, WT, false, WK>>(ta, tb, p, st))
     const int wk = (w_dtype == DT_I8) ? 0 : (w_dtype == DT_E4M3 ? 1 : (w_dtype == DT_E5M2 ? 2 : 3));
     if (a_dtype == DT_BF16) {
-      if (wk == 0) return QB_LAUNCH_BYTES(__nv_bfloat16, 0);
-      if (wk == 1) return QB_LAUNCH_BYTES(__nv_bfloat16, 1);
-      if (wk == 2) return QB_LAUNCH_BYTES(__nv_bfloat16, 2);
-      return QB_LAUNCH_BYTES(__nv_bfloat16, 3);
+      if (wk == 0) return QB_LAUNCH_BYTES(MmaKind::BF16, __nv_bfloat16, 0);
+      if (wk == 1) return QB_LAUNCH_BYTES(MmaKind::BF16, __nv_bfloat16, 1);
+      if (wk == 2) return QB_LAUNCH_BYTES(MmaKind::BF16, __nv_bfloat16, 2);
+      return QB_LAUNCH_BYTES(MmaKind::BF16, __nv_bfloat16, 3);
     }
-    if (wk == 0) return QB_LAUNCH_BYTES(__half, 0);
-    if (wk == 1) return QB_LAUNCH_BYTES(__half, 1);
-    if (wk == 2) return QB_LAUNCH_BYTES(__half, 2);
-    return QB_LAUNCH_BYTES(__half, 3);
+    if (wk == 0) return QB_LAUNCH_BYTES(MmaKind::F16, __half, 0);
+    if (wk == 1) return QB_LAUNCH_BYTES(MmaKind::F16, __half, 1);
+    if (wk == 2) return QB_LAUNCH_BYTES(MmaKind::F16, __half, 2);
+    return QB_LAUNCH_BYTES(MmaKind::F16, __half, 3);
 #undef QB_LAUNCH_BYTES
   }
   set_kernel_family(2);

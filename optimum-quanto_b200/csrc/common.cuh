@@ -1,9 +1,8 @@
-// Blackwell (sm_100a) device-side building blocks: mbarrier, TMA, tcgen05/TMEM wrappers and the
-// UMMA descriptor encodings used by every tensor-core kernel in this library.
+// Hopper (sm_90a) device-side building blocks: mbarrier, TMA, wgmma wrappers and the shared-memory
+// descriptor encoding used by every tensor-core kernel in this library.
 //
-// Everything here is inline PTX written against the PTX ISA 8.7 tcgen05 / cp.async.bulk.tensor
-// definitions; the bit layouts of the shared-memory and instruction descriptors are documented at
-// each encoder.  No CUTLASS/CuTe dependency.
+// Everything here is inline PTX written against the PTX ISA wgmma / cp.async.bulk.tensor definitions;
+// the bit layout of the shared-memory descriptor is documented at its encoder.  No CUTLASS/CuTe dependency.
 #pragma once
 
 #include <cuda.h>
@@ -12,6 +11,8 @@
 #include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 namespace qb {
 
@@ -29,7 +30,7 @@ enum : int { DT_F32 = 0, DT_F16 = 1, DT_BF16 = 2, DT_I8 = 3, DT_U8 = 4, DT_E4M3 
 #define QB_KO(flags, bit) false
 #endif
 
-constexpr int kNumSMsB200 = 148;
+constexpr int kNumSMsH100 = 132;  // H100 SXM
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -57,19 +58,6 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 // mbarrier
 // ------------------------------------------------------------------------------------------------
 // 32-bit-address flavours (the hot loops keep barrier addresses as integers)
-__device__ __forceinline__ bool mbar_try_wait_u32(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
 __device__ __forceinline__ void mbar_arrive_u32(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
@@ -87,37 +75,36 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
 }
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// Bounded wait: a protocol bug must surface as a trapped launch (cudaErrorLaunchFailure), never as a
-// hung GPU.  The watchdog only engages after many failed probes, so the fast path is one try_wait.
+// Bounded wait: a protocol bug must surface as a trapped launch (cudaErrorLaunchFailure), never as a hung GPU.  The whole
+// loop is one PTX block: a C++ spin loop is a thread-divergent branch, and one between two wgmma groups of a warpgroup
+// makes ptxas serialise the wgmma instructions (C7518).
 #ifndef QB_WATCHDOG_NS
 #define QB_WATCHDOG_NS 4000000000ull
 #endif
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  uint32_t probes = 0;
-  uint64_t t0 = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if (++probes == 4096u) {
-      uint64_t now = global_timer_ns();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > QB_WATCHDOG_NS) __trap();
-      probes = 0;
-    }
-  }
+__device__ __forceinline__ void mbar_wait_u32(uint32_t bar, uint32_t parity) {
+  // the clock is read once per 4096 failed probes (the first read starts the watchdog)
+  asm volatile(
+      "{\n.reg .pred p;\n.reg .u32 n;\n.reg .u64 t0, t1;\n"
+      "mov.u32 n, 0;\n"
+      "mov.u64 t0, 0;\n"
+      "WAIT_%=:\n"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+      "@p bra DONE_%=;\n"
+      "add.u32 n, n, 1;\n"
+      "and.b32 n, n, 4095;\n"
+      "setp.ne.u32 p, n, 0;\n"
+      "@p bra WAIT_%=;\n"
+      "mov.u64 t1, %%globaltimer;\n"
+      "setp.eq.u64 p, t0, 0;\n"
+      "@p mov.u64 t0, t1;\n"
+      "sub.u64 t1, t1, t0;\n"
+      "setp.lt.u64 p, t1, %2;\n"
+      "@p bra WAIT_%=;\n"
+      "trap;\n"
+      "DONE_%=:\n}\n" ::"r"(bar), "r"(parity), "l"(QB_WATCHDOG_NS)
+      : "memory");
 }
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) { mbar_wait_u32(smem_u32(bar), parity); }
 
 // explicit shared-space accesses on 32-bit shared addresses (generic-pointer stores compile to slower ST/LD)
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
@@ -129,21 +116,7 @@ __device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
   return v;
 }
 
-__device__ __forceinline__ void mbar_wait_u32(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait_u32(bar, parity)) return;
-  uint32_t probes = 0;
-  uint64_t t0 = 0;
-  while (!mbar_try_wait_u32(bar, parity)) {
-    if (++probes == 4096u) {
-      uint64_t now = global_timer_ns();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > QB_WATCHDOG_NS) __trap();
-      probes = 0;
-    }
-  }
-}
-
-// generic-proxy writes (st.shared) -> visible to the async proxy (tcgen05.mma / TMA reads)
+// generic-proxy writes (st.shared) -> visible to the async proxy (wgmma / TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -162,127 +135,172 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
+// bulk async-group bookkeeping of shared -> global bulk copies
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+__device__ __forceinline__ void bulk_wait_group_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
 // ------------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA issue, commit, TMEM loads
+// wgmma (Hopper warpgroup MMA): D[64 x N] (+)= A[64 x K] * B[N x K]^T, both operands K-major in shared memory,
+// accumulators in the registers of the issuing warpgroup.  Fragment of thread t (warp w = t / 32 of the
+// warpgroup, lane l): d[4 j + 2 h + e] holds row 16 w + l / 4 + 8 h, column 8 j + 2 (l % 4) + e.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {  // whole warp, .sync.aligned
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// All previously issued tcgen05.mma of this thread arrive (count 1) on `bar` when they complete.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-enum class MmaKind { F16, I8, F8F6F4 };
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; single-thread issue.
-template <MmaKind K>
-__device__ __forceinline__ void tc_mma(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                       uint32_t accumulate) {
-  if constexpr (K == MmaKind::F16) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else if constexpr (K == MmaKind::I8) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+// Keeps the compiler from moving accumulator reads / writes across an in-flight wgmma.
+template <typename T, int N>
+__device__ __forceinline__ void wgmma_fence_operands(T (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) {
+    if constexpr (sizeof(T) == 4 && std::is_same<T, float>::value) asm volatile("" : "+f"(d[i])::"memory");
+    else asm volatile("" : "+r"(d[i])::"memory");
   }
 }
 
-// D[tmem] (+)= A[tmem] * B[smem desc]: the A operand (M = 128 lanes, K elements packed two bf16/fp16 per 32-bit
-// column, 8 columns per K = 16 step) is read from tensor memory instead of shared memory.  Measured on B200:
-// 46 cycles per M=128 instruction for N <= 64 (88 with A in shared memory), 64 at N = 128, 128 at N = 256.
-__device__ __forceinline__ void tc_mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// registers -> TMEM: lane i of the warp writes 32 consecutive columns of TMEM lane (32*(warp%4) + i)
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,"
-      "%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-// 8 columns (one 16-k chunk of an A operand in tensor memory): lane i of the warp writes TMEM lane 32*(warp%4) + i
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-               "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// Warp w may touch TMEM lanes [32*(w%4), 32*(w%4)+32). 32x32b.x16: lane i <- TMEM lane base+i, 16 columns.
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------------------------------------
-// UMMA descriptors
-// ------------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (64 bit), K-major operand stored as rows of 128 bytes with the
-// 128-byte swizzle (16-byte chunk index XOR (row & 7)), 8-row groups 1024 bytes apart:
-//   [ 0,14)  start address  >> 4
-//   [16,30)  leading-dim byte offset >> 4   (ignored for swizzled K-major; set to 1)
-//   [32,46)  stride-dim  byte offset >> 4   (distance between 8-row groups = 1024 B -> 64)
-//   [46,48)  descriptor version = 1 on sm_100
+// Shared-memory matrix descriptor (64 bit) of a K-major operand stored as rows of 128 bytes with the 128-byte
+// swizzle (16-byte chunk index XOR (row & 7)), 8-row groups 1024 bytes apart -- what TMA writes with
+// CU_TENSOR_MAP_SWIZZLE_128B:
+//   [ 0,14)  start address >> 4   (a K step inside the 128-byte row advances it by the step's bytes)
+//   [16,30)  leading-dim byte offset >> 4 (unused for swizzled K-major layouts; 1)
+//   [32,46)  stride-dim byte offset >> 4  (distance between 8-row groups = 1024 B -> 64)
 //   [49,52)  base offset = 0 (tiles are 1024-byte aligned)
-//   [61,64)  layout type: 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t umma_desc_sw128_kmajor(uint32_t smem_addr) {
+//   [62,64)  layout type: 1 = SWIZZLE_128B
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// Instruction descriptor (32 bit) for kind::f16 / kind::i8 / kind::f8f6f4, dense, K-major A and B:
-//   [4,6)   D format: 0 f16, 1 f32, 2 s32
-//   [7,10)  A format   [10,13) B format   (f16: 0 f16 / 1 bf16; i8: 0 u8 / 1 s8; f8f6f4: 0 e4m3 / 1 e5m2)
-//   [15]    A major (0 = K)  [16] B major (0 = K)
-//   [17,23) N >> 3     [24,29) M >> 4
-__host__ __device__ constexpr uint32_t umma_idesc(uint32_t d_fmt, uint32_t a_fmt, uint32_t b_fmt, uint32_t m,
-                                                  uint32_t n) {
-  return (d_fmt << 4) | (a_fmt << 7) | (b_fmt << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
+enum class MmaKind { F16, BF16, I8 };
+
+
+// bf16 x bf16 -> f32, N = 128, K = 16 (32 bytes of each operand row)
+__device__ __forceinline__ void wgmma_bf16_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{" 
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
+// fp16 x fp16 -> f32, N = 128, K = 16
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{" 
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
+// int8 x int8 -> s32 (exact), N = 128, K = 32
+__device__ __forceinline__ void wgmma_s8_n128(uint32_t (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+      "{" 
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p;\n}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+        "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+        "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+        "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+        "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+        "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+        "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
+// int8 x int8 -> s32 (exact), N = 256, K = 32
+__device__ __forceinline__ void wgmma_s8_n256(uint32_t (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 "
+      "{" 
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p;\n}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+        "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+        "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+        "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+        "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+        "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+        "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]),
+        "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]),
+        "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]),
+        "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]),
+        "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]),
+        "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]),
+        "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]),
+        "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]),
+        "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+
+
+// One MMA K step (32 bytes of each operand row) of a 64-row A panel against a BN-row B tile, dispatched on the kind.
+template <MmaKind KA, int BN, typename T, int NACC>
+__device__ __forceinline__ void wgmma_step(T (&d)[NACC], uint32_t a_addr, uint32_t b_addr, uint32_t acc) {
+  const uint64_t da = wgmma_desc_sw128(a_addr), db = wgmma_desc_sw128(b_addr);
+  if constexpr (KA == MmaKind::BF16) wgmma_bf16_n128(d, da, db, acc);
+  else if constexpr (KA == MmaKind::F16) wgmma_f16_n128(d, da, db, acc);
+  else if constexpr (KA == MmaKind::I8 && BN == 256) wgmma_s8_n256(d, da, db, acc);
+  else wgmma_s8_n128(d, da, db, acc);
+}
+
+// One 128-byte K slab (4 MMA K steps).
+template <MmaKind KA, int BN, typename T, int NACC>
+__device__ __forceinline__ void wgmma_slab(T (&d)[NACC], uint32_t a_addr, uint32_t b_addr, bool accumulate_first) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    wgmma_step<KA, BN>(d, a_addr + k * 32, b_addr + k * 32, (k > 0 || accumulate_first) ? 1u : 0u);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -14,7 +14,7 @@ constexpr int kEwThreads = 256;
 
 static inline int ew_grid(int64_t work_items) {
   int64_t blocks = (work_items + kEwThreads - 1) / kEwThreads;
-  int64_t cap = static_cast<int64_t>(kNumSMsB200) * 16;  // 16 resident CTAs of 256 threads cover 2048 thr/SM x2 waves
+  int64_t cap = static_cast<int64_t>(kNumSMsH100) * 16;  // 16 resident CTAs of 256 threads cover 2048 thr/SM x2 waves
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   return static_cast<int>(blocks);

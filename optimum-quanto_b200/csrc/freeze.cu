@@ -24,7 +24,7 @@ constexpr int kFzThreads = 256;
 
 static inline int fz_grid(int64_t threads_needed, int ctas_per_sm) {
   int64_t blocks = (threads_needed + kFzThreads - 1) / kFzThreads;
-  const int64_t cap = static_cast<int64_t>(kNumSMsB200) * ctas_per_sm;
+  const int64_t cap = static_cast<int64_t>(kNumSMsH100) * ctas_per_sm;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   return static_cast<int>(blocks);
@@ -537,7 +537,7 @@ template <typename T>
 static int launch_qqa(const void* base, void* out, void* scale, int64_t n, int64_t k, int out_dt, cudaStream_t stream) {
   const int vec_ok = (k % 8 == 0) && (reinterpret_cast<uintptr_t>(base) % 16 == 0) &&
                      (reinterpret_cast<uintptr_t>(out) % 8 == 0);
-  const int grid = static_cast<int>(n < static_cast<int64_t>(kNumSMsB200) * 8 ? n : static_cast<int64_t>(kNumSMsB200) * 8);
+  const int grid = static_cast<int>(n < static_cast<int64_t>(kNumSMsH100) * 8 ? n : static_cast<int64_t>(kNumSMsH100) * 8);
   const T* b = static_cast<const T*>(base);
   uint8_t* o = static_cast<uint8_t*>(out);
   T* s = static_cast<T*>(scale);

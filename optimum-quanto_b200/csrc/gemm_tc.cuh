@@ -1,20 +1,20 @@
-// Persistent, warp-specialised tcgen05 GEMM for the quantized-linear forward.
+// Persistent, warp-specialised wgmma GEMM for the quantized-linear forward (Hopper, sm_90a).
 //
 //   out[m, n] = epilogue( sum_k A[m, k] * Wt[n, k] )
 //
-// One CTA per SM loops over output tiles.  Roles (one warp each unless noted):
-//   warp 0      TMA producer   : A tiles (and W tiles when W is 8-bit and fed straight to the tensor core)
-//   warp 1      MMA issuer     : one elected thread issues tcgen05.mma, accumulators live in TMEM
-//   warps 2-5   epilogue       : tcgen05.ld TMEM -> registers -> scale / bias / round -> global
-//   warps 6-13  weight staging : (int4 / mixed paths only) vector-load the packed uint8 weight bytes, unpack,
-//                                apply the per-group scale/shift with the reference's exact rounding order and
-//                                write the bf16/fp16 tile into shared memory in the 128B-swizzled K-major
-//                                layout the tensor core reads -- no separate dequantise launch, the
-//                                dequantised weight never exists in HBM.
+// One CTA per SM loops over BM x BN output tiles (BM = 64 per consumer warpgroup, BN = 128 or 256).  Roles:
+//   warps [0, 4*MWG)  consumers      : one warpgroup per 64 rows of the tile issues wgmma (accumulators in registers)
+//                                      and runs the epilogue (scale / bias / round / optional output quantisation)
+//   warp 4*MWG        TMA producer   : A tiles (and W tiles when W is 8-bit and fed straight to the tensor core)
+//   further warps     weight staging : (int4 / weight-only 8-bit) vector-load the packed weight bytes, unpack,
+//                                      apply the per-group scale/shift with the reference's exact rounding order and
+//                                      write the bf16/fp16 tile into shared memory in the 128B-swizzled K-major
+//                                      layout the tensor core reads -- no separate dequantise launch, the
+//                                      dequantised weight never exists in HBM.
 //
 // Shared-memory operand layout (both operands, K-major): a tile is `rows x 128 bytes`; row r lives at
 // (r/8)*1024 + (r%8)*128 and its 16-byte chunk c is stored at chunk position c ^ (r%8)  (SWIZZLE_128B, the
-// layout TMA produces and the UMMA descriptor in common.cuh describes).
+// layout TMA produces and the wgmma descriptor in common.cuh describes).
 #pragma once
 
 #include <type_traits>
@@ -25,7 +25,9 @@
 
 namespace qb {
 
-enum class BSrc { TMA, INT4, BYTES };  // BYTES: int8 / fp8 weights converted in-kernel to the activation dtype
+// BYTES: int8 / fp8 weights converted in-kernel to the activation dtype; F8: fp8 activations AND weights converted
+// in-kernel to bf16 (exact: every e4m3 / e5m2 value is a bf16 value), so that the products are exact and summed in fp32
+enum class BSrc { TMA, INT4, BYTES, F8 };
 
 struct GemmParams {
   // epilogue
@@ -53,75 +55,13 @@ struct GemmParams {
   // activation dtype; the staging warps write rnd(scale * W) exactly as the reference's python path does
   // (library/qbytes_mm.py:25-33), so the GEMM operands are bit-identical to the reference's
   int w_dt;
+  const void* a;       // F8 only: the [M, K] fp8 activations, read by the staging warps
   // Fused output quantisation (SURVEY 8f rank 2: QModuleMixin.quantize_output, nn/qmodule.py:300-302, fused into the
   // epilogue): q_dt = DT_I8 / DT_E4M3 / DT_E5M2 (0 = off), q_scale = DEVICE pointer to the per-tensor output scale in
   // `out_dt`.  The result rounded to out_dt (+ bias, rounded) is divided by the scale in out_dt, rounded, clamped and
   // cast exactly like quanto::quantize_symmetric; `out` is then a [M, ld] buffer of BYTES.
   int q_dt;
   const void* q_scale;
-  long long* trace;    // developer timeline (tools/trace_gemm.py) or nullptr
-  int dbg;             // developer knock-out flags (pair kernel: 64 skip epilogue math/stores, 128 L2-hot operand loads)
-};
-
-// developer timeline: CTA < 4 records up to 64 clock64 stamps per role (0 TMA producer, 2 MMA, 3 epilogue,
-// 4 staging group 0 lane 0).  One uniform branch per call when disabled.
-__device__ __forceinline__ void gemm_trace_evt(const GemmParams& p, int role, int& n) {
-  if (p.trace != nullptr && blockIdx.x < 4 && n < 64) {
-    p.trace[(static_cast<size_t>(blockIdx.x) * 5 + role) * 64 + n] = clock64();
-    ++n;
-  }
-}
-
-// per-tile, per-column epilogue operands staged in shared memory as fp32 (see epi_stage_cols)
-struct EpiCols {
-  float sc[2][256];  // [tile parity][tile column]
-  float bi[2][256];
-};
-
-// TMA store descriptors of the EPI = 1 epilogue: one [M, ld] view per output buffer (kernel parameter, 1 KB)
-struct StoreMaps {
-  CUtensorMap m[kMaxGatherWorld];
-};
-
-// EPI_: how the epilogue leaves the SM.  0 = every lane stores its own row chunk (st.global); 1 = the warp stages a
-// 32-row x 64-column block in shared memory (128-byte swizzle) and ONE thread hands it to the TMA store unit, once per
-// output buffer (this rank's, and its peers' for the fused all-gather): full 128-byte rows per request instead of 32
-// scattered 32-byte pieces -- what NVLink needs -- and a handful of instructions per block instead of hundreds.
-template <MmaKind KIND_, BSrc BSRC_, int MSUB_, int BN_, typename WT_, bool ZP_ = false, int WKIND_ = 0, int EPI_ = 0>
-struct GemmCfg {
-  static constexpr int EPI = EPI_;
-  static constexpr bool ZP = ZP_;     // INT4 only: shift is an integer zero-point (compile-time: keeps the hot loop lean)
-  static constexpr int WKIND = WKIND_;  // BYTES only: 0 int8, 1 float8_e4m3fn, 2 float8_e5m2, 3 float8_e4m3fnuz
-  static constexpr MmaKind KIND = KIND_;
-  static constexpr BSrc BSRC = BSRC_;
-  static constexpr int MSUB = MSUB_;  // 128-row A sub-tiles per CTA tile (B tile reused across them)
-  static constexpr int BN = BN_;      // UMMA N
-  using WT = WT_;                     // element type of the staged weight tile (bf16 / half), INT4 only
-  static constexpr int BM = 128;      // UMMA M (cta_group::1)
-  static constexpr int KBYTES = 128;  // K extent of one pipeline stage in bytes = one swizzle atom
-  static constexpr int A_TILE = BM * KBYTES;
-  static constexpr int B_TILE = BN * KBYTES;
-  static constexpr int STAGE = MSUB * A_TILE + B_TILE;
-  static constexpr int NSTAGES = (196 * 1024) / STAGE;
-  static constexpr int ACC_COLS = MSUB * BN;
-  static constexpr int NACC = (2 * ACC_COLS <= 512) ? 2 : 1;
-  static constexpr int TMEM_COLS = 512;
-  // INT4 staging: one group of BN/64 warps (one thread per packed row) per pipeline stage slot; group g converts
-  // the stages it == g (mod NSTAGES) into slot g, so NSTAGES stages are being converted concurrently and every
-  // thread amortises its per-stage overhead over a full 64-k row (128 weights).
-  static constexpr int CVT_GROUP_WARPS = (BN / 2 + 31) / 32;  // INT4: one thread per packed row (BN = 224: the last
-                                                               // warp is half idle) ; BYTES: two weight rows per thread
-  static constexpr int NCVT_WARPS = (BSRC == BSrc::TMA) ? 0 : NSTAGES * CVT_GROUP_WARPS;
-  static constexpr int NCVT_THREADS = NCVT_WARPS * 32;
-  static constexpr int FULL_ARRIVALS = 1 + ((BSRC == BSrc::TMA) ? 0 : CVT_GROUP_WARPS);
-  static constexpr int NTHREADS = (6 + NCVT_WARPS) * 32;
-  static constexpr int EPI_STAGE_BYTES = (EPI == 1) ? 4 * 2 * 4096 : 0;  // 4 epilogue warps x 2 buffers x (32 rows x 128 B)
-  // dynamic shared memory is declared __align__(1024) (checked at kernel entry), so no alignment slack is reserved
-  static constexpr int SMEM_BYTES = NSTAGES * STAGE + EPI_STAGE_BYTES + 256 /*barriers*/ + ((EPI == 1) ? 2048 /*bias, two tile parities*/ : static_cast<int>(sizeof(EpiCols)));
-  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-  static_assert(EPI == 0 || (BN / 2) % 64 == 0, "TMA-store epilogue: both nibble halves of the tile are whole 64-column blocks");
-  static_assert(ACC_COLS * NACC <= 512, "TMEM overflow");
-  static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256, "invalid UMMA N");
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -348,65 +288,51 @@ __device__ __forceinline__ void stage_row_64k(const uint4 (&raw)[4], uint32_t s2
   }
 }
 
-// Epilogue for one 16-column chunk held by one thread (= one output row).
-template <typename OT, bool IS_INT_ACC>
-__device__ __forceinline__ void epilogue_store16(const uint32_t (&v)[16], OT* __restrict__ out_row, int n_first,
-                                                 int n_limit, bool row_ok, const OT* __restrict__ scales,
-                                                 const OT* __restrict__ bias, bool vec_ok) {
-  alignas(16) OT o[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    float f = IS_INT_ACC ? __int2float_rn(static_cast<int>(v[j])) : __uint_as_float(v[j]);
-    const int n = n_first + j;
-    if (scales != nullptr && n < n_limit) f = __fmul_rn(f, to_float<OT>(scales[n]));
-    OT r = from_float<OT>(f);
-    if (bias != nullptr && n < n_limit) r = from_float<OT>(__fadd_rn(to_float<OT>(r), to_float<OT>(bias[n])));
-    o[j] = r;
-  }
-  if (!row_ok) return;
-  if (vec_ok && n_first + 16 <= n_limit) {
-    uint4* dst = reinterpret_cast<uint4*>(out_row + n_first);
-    const uint4* src = reinterpret_cast<const uint4*>(o);
-#pragma unroll
-    for (int q = 0; q < static_cast<int>(sizeof(OT) * 16 / 16); ++q) dst[q] = src[q];
-  } else {
-#pragma unroll
-    for (int j = 0; j < 16; ++j)
-      if (n_first + j < n_limit) out_row[n_first + j] = o[j];
-  }
-}
-
-// Fast path of the epilogue: a full, aligned 16-column chunk of an fp32 accumulator with no scale / bias.
-template <typename OT>
-__device__ __forceinline__ void epilogue_store16_plain(const uint32_t (&v)[16], OT* __restrict__ dst) {
-  if constexpr (sizeof(OT) == 2) {
-    uint32_t o[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      if constexpr (std::is_same<OT, __nv_bfloat16>::value) {
-        __nv_bfloat162 t = __floats2bfloat162_rn(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
-        o[j] = *reinterpret_cast<uint32_t*>(&t);
-      } else {
-        __half2 t = __floats2half2_rn(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
-        o[j] = *reinterpret_cast<uint32_t*>(&t);
-      }
-    }
-    uint4* d = reinterpret_cast<uint4*>(dst);
-    d[0] = make_uint4(o[0], o[1], o[2], o[3]);
-    d[1] = make_uint4(o[4], o[5], o[6], o[7]);
-  } else {
-    uint4* d = reinterpret_cast<uint4*>(dst);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) d[q] = make_uint4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-  }
-}
+// ------------------------------------------------------------------------------------------------
+// Kernel configuration
+// ------------------------------------------------------------------------------------------------
+// KIND_: MMA operand kind (F16 / BF16, or I8 for int8 x int8).  MWG_: consumer warpgroups (BM = 64 * MWG_).
+// WT_: staged element type (INT4 / BYTES / F8).
+template <MmaKind KIND_, BSrc BSRC_, int MWG_, int BN_, typename WT_ = __nv_bfloat16, bool ZP_ = false, int WKIND_ = 0,
+          int AKIND_ = 0>
+struct GemmCfg {
+  static constexpr MmaKind KIND = KIND_;
+  static constexpr BSrc BSRC = BSRC_;
+  static constexpr bool ZP = ZP_;       // INT4 only: shift is an integer zero-point (compile-time: keeps the hot loop lean)
+  static constexpr int WKIND = WKIND_;  // BYTES / F8: weight bytes: 0 int8, 1 float8_e4m3fn, 2 float8_e5m2, 3 float8_e4m3fnuz
+  static constexpr int AKIND = AKIND_;  // F8: activation bytes, same codes
+  using WT = WT_;
+  static constexpr int MWG = MWG_;
+  static constexpr int BM = 64 * MWG;
+  static constexpr int BN = BN_;
+  static constexpr bool IS_INT = (KIND == MmaKind::I8);
+  static constexpr int NACC = BN / 2;   // accumulator registers per consumer thread
+  static constexpr int KBYTES = 128;    // K extent of one pipeline stage in bytes = one swizzle atom
+  static constexpr int A_TILE = BM * KBYTES;
+  static constexpr int B_TILE = BN * KBYTES;
+  static constexpr int STAGE = A_TILE + B_TILE;
+  // staged weights: one staging group (BN/64 warps: one thread per packed int4 row, or per two 8-bit rows -- and for F8
+  // per one or two activation rows) per stage slot.  3 slots keep the CTA at 15 warps, which leaves 128 registers per thread (the consumers hold 64 accumulators).
+  static constexpr int CVT_GROUP_WARPS = BN / 64;
+  static constexpr int NSTAGES = (BSRC == BSrc::TMA) ? ((192 * 1024) / STAGE > 8 ? 8 : (192 * 1024) / STAGE) : 3;
+  static constexpr int NCVT_WARPS = (BSRC == BSrc::TMA) ? 0 : NSTAGES * CVT_GROUP_WARPS;
+  static constexpr int PRODUCER_WARP = 4 * MWG;
+  static constexpr int FIRST_CVT_WARP = PRODUCER_WARP + 1;
+  static constexpr int NTHREADS = (FIRST_CVT_WARP + NCVT_WARPS) * 32;
+  // the TMA producer's arrive (A tile, and W for TMA) + one per staging warp; F8 stages both operands without TMA
+  static constexpr int FULL_ARRIVALS = (BSRC == BSrc::F8 ? 0 : 1) + ((BSRC == BSrc::TMA) ? 0 : CVT_GROUP_WARPS);
+  // 1024 bytes of alignment slack (the swizzled tiles need 1024-byte aligned bases) + the barriers
+  static constexpr int SMEM_BYTES = 1024 + NSTAGES * STAGE + 2 * NSTAGES * 8;
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
+  static_assert(BN == 128 || (BN == 256 && IS_INT && BSRC == BSrc::TMA), "wgmma tile width");
+  static_assert(BSRC == BSrc::TMA || KIND == MmaKind::F16 || KIND == MmaKind::BF16, "staged weights are 16-bit");
+};
 
 // ------------------------------------------------------------------------------------------------
-// Epilogue with per-column scale / bias.  One epilogue warp runs alone on its SM sub-partition, so its cost is
-// instruction count x dependent-issue latency (measured: the predicated per-element version took ~2300 cycles per
-// 16-column chunk, twice the tile's MMA time).  The per-column scale and bias of the tile are therefore staged once
-// per tile into shared memory as fp32 (exact: they are fp16/bf16/fp32 values) and a chunk becomes
-// 16 I2F/FMUL + 8 packs + 8 LDS.128 + 2-4 STG.128 with full ILP.
+// Epilogue, one pair of adjacent accumulator columns of one output row (the wgmma fragment holds pairs):
+//   8-bit operands : rnd_OT(acc * scale[n]) (+ bias, rounded) -- the reference's qbytes_mm + bias order;
+//                    with q_dt != 0 that result is then quantised like quanto::quantize_symmetric and stored as bytes
+//   16-bit operands: rnd_OT(acc) (+ bias, rounded)
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float load_out_dt_as_float(const void* base, int dt, int i) {
   if (dt == DT_BF16) return __bfloat162float(static_cast<const __nv_bfloat16*>(base)[i]);
@@ -414,494 +340,212 @@ __device__ __forceinline__ float load_out_dt_as_float(const void* base, int dt, 
   return static_cast<const float*>(base)[i];
 }
 
-// called by the 128 epilogue threads (et = 0..127); col_to_n(c) -> output feature of tile column c, or -1
-template <class F>
-__device__ __forceinline__ void epi_stage_cols(EpiCols* ec, int buf, const GemmParams& p, int et, int ncols,
-                                               F col_to_n) {
-  for (int c = et; c < ncols; c += 128) {
-    const int n = col_to_n(c);
-    float sv = 1.f, bv = 0.f;
-    if (n >= 0) {
-      if (p.scales != nullptr) sv = load_out_dt_as_float(p.scales, p.out_dt, n);
-      if (p.bias != nullptr) bv = load_out_dt_as_float(p.bias, p.out_dt, n);
-    }
-    ec->sc[buf][c] = sv;
-    ec->bi[buf][c] = bv;
-  }
-  asm volatile("bar.sync 1, 128;" ::: "memory");  // the four epilogue warps only
-}
-
 template <typename OT>
-__device__ __forceinline__ float2 unpack2(uint32_t v);
-template <>
-__device__ __forceinline__ float2 unpack2<__nv_bfloat16>(uint32_t v) {
-  return make_float2(__uint_as_float(v << 16), __uint_as_float(v & 0xFFFF0000u));
-}
-template <>
-__device__ __forceinline__ float2 unpack2<__half>(uint32_t v) {
-  return __half22float2(*reinterpret_cast<__half2*>(&v));
-}
-
-// One full, 16-byte-aligned 16-column chunk: acc -> fp32 -> * scale -> round to OT -> + bias -> round to OT
-// (the rounding order of the reference: qbytes_mm output rounded to the scales' dtype, bias added by the caller).
-template <typename OT, bool IS_INT>
-__device__ __forceinline__ void epilogue_chunk_fast(const uint32_t (&v)[16], uint32_t sc_addr, uint32_t bi_addr,
-                                                    bool has_scale, bool has_bias, OT* __restrict__ dst) {
-  float f[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) f[j] = IS_INT ? __int2float_rn(static_cast<int>(v[j])) : __uint_as_float(v[j]);
-  if (has_scale) {
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const uint4 sv = ld_shared_v4(sc_addr + q * 16);
-      f[4 * q + 0] = __fmul_rn(f[4 * q + 0], __uint_as_float(sv.x));
-      f[4 * q + 1] = __fmul_rn(f[4 * q + 1], __uint_as_float(sv.y));
-      f[4 * q + 2] = __fmul_rn(f[4 * q + 2], __uint_as_float(sv.z));
-      f[4 * q + 3] = __fmul_rn(f[4 * q + 3], __uint_as_float(sv.w));
-    }
-  }
-  if constexpr (sizeof(OT) == 2) {
-    uint32_t o[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) o[j] = pack2<OT>(f[2 * j], f[2 * j + 1]);
-    if (has_bias) {
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const uint4 bv = ld_shared_v4(bi_addr + q * 16);
-        const float2 a = unpack2<OT>(o[2 * q]), b = unpack2<OT>(o[2 * q + 1]);
-        o[2 * q] = pack2<OT>(__fadd_rn(a.x, __uint_as_float(bv.x)), __fadd_rn(a.y, __uint_as_float(bv.y)));
-        o[2 * q + 1] = pack2<OT>(__fadd_rn(b.x, __uint_as_float(bv.z)), __fadd_rn(b.y, __uint_as_float(bv.w)));
-      }
-    }
-    uint4* d = reinterpret_cast<uint4*>(dst);
-    d[0] = make_uint4(o[0], o[1], o[2], o[3]);
-    d[1] = make_uint4(o[4], o[5], o[6], o[7]);
+__device__ __forceinline__ void store_pair(OT* dst, float a, float b, bool two, bool vec) {
+  if (two && vec) {
+    if constexpr (sizeof(OT) == 2) *reinterpret_cast<uint32_t*>(dst) = pack2<OT>(a, b);
+    else *reinterpret_cast<float2*>(dst) = make_float2(a, b);
   } else {
-    if (has_bias) {
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const uint4 bv = ld_shared_v4(bi_addr + q * 16);
-        f[4 * q + 0] = __fadd_rn(f[4 * q + 0], __uint_as_float(bv.x));
-        f[4 * q + 1] = __fadd_rn(f[4 * q + 1], __uint_as_float(bv.y));
-        f[4 * q + 2] = __fadd_rn(f[4 * q + 2], __uint_as_float(bv.z));
-        f[4 * q + 3] = __fadd_rn(f[4 * q + 3], __uint_as_float(bv.w));
-      }
-    }
-    uint4* d = reinterpret_cast<uint4*>(dst);
-#pragma unroll
-    for (int q = 0; q < 4; ++q)
-      d[q] = make_uint4(__float_as_uint(f[4 * q]), __float_as_uint(f[4 * q + 1]), __float_as_uint(f[4 * q + 2]),
-                        __float_as_uint(f[4 * q + 3]));
+    dst[0] = from_float<OT>(a);
+    if (two) dst[1] = from_float<OT>(b);
   }
 }
 
-// One 16-column chunk of one output row, any case: plain / staged fast path / ragged element-wise path.
-//   col0: first tile column of the chunk (index into the staged scale / bias), n_first: its output feature.
-// One 16-column chunk of one output row, any case: plain / staged fast path / ragged element-wise path, stored into
-// one output buffer.
-//   col0: first tile column of the chunk (index into the staged scale / bias), n_first: its (local) output feature.
-// Quantised-output epilogue of one 16-column chunk: y = rnd_OT(acc * scale) (+ bias, rounded) as in the ordinary
-// epilogue, then quantize_symmetric(y, out_scale) (library/quantize.py:51-55: rnd_OT(y / s), rint / clamp / cast) and one
-// 16-byte store.  Per-column scale / bias come from the staged fp32 copies (always staged: scales is never null here).
-template <typename OT, int QDT, bool IS_INT>
-__device__ __forceinline__ void epilogue_quant16(const GemmParams& p, uint8_t* __restrict__ out_row,
-                                                 const uint32_t (&v)[16], int n_first, int n_limit, const EpiCols* ec,
-                                                 int buf, int col0) {
-  const float qs = to_float<OT>(*static_cast<const OT*>(p.q_scale));
-  const bool fast = rcp_is_safe<OT>(qs);
-  const float qr = fast ? __frcp_rn(qs) : 0.f;
-  float y[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    const float f = IS_INT ? __int2float_rn(static_cast<int>(v[j])) : __uint_as_float(v[j]);
-    y[j] = __fmul_rn(f, ec->sc[buf][col0 + j]);
+// f0, f1: accumulator values of output features n, n + 1 (n + 1 only when `two`); row_off = row * ld + col0.
+template <typename OT, bool ALLOW_Q>
+__device__ __forceinline__ void epilogue_pair_t(const GemmParams& p, size_t row_off, int n, bool two, float f0, float f1) {
+  if (p.scales != nullptr) {
+    f0 = __fmul_rn(f0, load_out_dt_as_float(p.scales, p.out_dt, n));
+    if (two) f1 = __fmul_rn(f1, load_out_dt_as_float(p.scales, p.out_dt, n + 1));
   }
-#pragma unroll
-  for (int j = 0; j < 16; j += 2) rnd_pair<OT>(y[j], y[j + 1]);
+  rnd_pair<OT>(f0, f1);
   if (p.bias != nullptr) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) y[j] = __fadd_rn(y[j], ec->bi[buf][col0 + j]);
-#pragma unroll
-    for (int j = 0; j < 16; j += 2) rnd_pair<OT>(y[j], y[j + 1]);
+    f0 = __fadd_rn(f0, load_out_dt_as_float(p.bias, p.out_dt, n));
+    if (two) f1 = __fadd_rn(f1, load_out_dt_as_float(p.bias, p.out_dt, n + 1));
+    rnd_pair<OT>(f0, f1);
   }
-  if (fast) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) y[j] = __fmul_rn(y[j], qr);
-  } else {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) y[j] = __fdiv_rn(y[j], qs);
-  }
-#pragma unroll
-  for (int j = 0; j < 16; j += 2) rnd_pair<OT>(y[j], y[j + 1]);
-  alignas(16) uint8_t q[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) q[j] = quantize_one<QDT>(y[j]);
-  uint8_t* dst = out_row + n_first;
-  if (n_first + 16 <= n_limit && (reinterpret_cast<uintptr_t>(dst) % 16 == 0)) {
-    *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(q);
-  } else {
-#pragma unroll
-    for (int j = 0; j < 16; ++j)
-      if (n_first + j < n_limit) dst[j] = q[j];
-  }
-}
-
-template <typename OT, bool IS_INT>
-__device__ __forceinline__ void epilogue_quant16_dt(const GemmParams& p, uint8_t* out_row, const uint32_t (&v)[16],
-                                                    int n_first, int n_limit, const EpiCols* ec, int buf, int col0) {
-  if (p.q_dt == DT_I8) epilogue_quant16<OT, DT_I8, IS_INT>(p, out_row, v, n_first, n_limit, ec, buf, col0);
-  else if (p.q_dt == DT_E4M3) epilogue_quant16<OT, DT_E4M3, IS_INT>(p, out_row, v, n_first, n_limit, ec, buf, col0);
-  else epilogue_quant16<OT, DT_E5M2, IS_INT>(p, out_row, v, n_first, n_limit, ec, buf, col0);
-}
-
-// ALLOW_Q: compiled only into the int8 / fp8 kernels (the ones quanto::qbytes_mm with quantized activations runs), so the
-// fp16 / bf16 kernels carry neither the branch nor its registers.
-template <bool IS_INT, bool ALLOW_Q>
-__device__ __forceinline__ void epilogue_chunk_to(const GemmParams& p, void* out, const uint32_t (&v)[16], int row,
-                                                  int n_first, int n_limit, bool plain, const EpiCols* ec, int buf,
-                                                  int col0) {
-  const size_t row_off = static_cast<size_t>(row) * p.ld + p.col0;
-  if (ALLOW_Q && p.q_dt != 0) {
-    uint8_t* out_row = static_cast<uint8_t*>(out) + row_off;
-    if (p.out_dt == DT_BF16) epilogue_quant16_dt<__nv_bfloat16, IS_INT>(p, out_row, v, n_first, n_limit, ec, buf, col0);
-    else if (p.out_dt == DT_F16) epilogue_quant16_dt<__half, IS_INT>(p, out_row, v, n_first, n_limit, ec, buf, col0);
-    else epilogue_quant16_dt<float, IS_INT>(p, out_row, v, n_first, n_limit, ec, buf, col0);
-    return;
-  }
-  const int esz = (p.out_dt == DT_F32) ? 4 : 2;
-  const bool full = (n_first + 16 <= n_limit) && (((row_off + n_first) * esz) % 16 == 0);
-  if (full) {
-    if (plain) {
-      if (p.out_dt == DT_BF16) epilogue_store16_plain(v, static_cast<__nv_bfloat16*>(out) + row_off + n_first);
-      else if (p.out_dt == DT_F16) epilogue_store16_plain(v, static_cast<__half*>(out) + row_off + n_first);
-      else epilogue_store16_plain(v, static_cast<float*>(out) + row_off + n_first);
+  if constexpr (ALLOW_Q) {
+    if (p.q_dt != 0) {
+      const float qs = to_float<OT>(*static_cast<const OT*>(p.q_scale));
+      if (rcp_is_safe<OT>(qs)) {
+        const float qr = __frcp_rn(qs);
+        f0 = __fmul_rn(f0, qr);
+        f1 = __fmul_rn(f1, qr);
+      } else {
+        f0 = __fdiv_rn(f0, qs);
+        f1 = __fdiv_rn(f1, qs);
+      }
+      rnd_pair<OT>(f0, f1);
+      uint8_t q0, q1;
+      if (p.q_dt == DT_I8) { q0 = quantize_one<DT_I8>(f0); q1 = quantize_one<DT_I8>(f1); }
+      else if (p.q_dt == DT_E4M3) { q0 = quantize_one<DT_E4M3>(f0); q1 = quantize_one<DT_E4M3>(f1); }
+      else { q0 = quantize_one<DT_E5M2>(f0); q1 = quantize_one<DT_E5M2>(f1); }
+      for (int q = 0; q < p.g.n_out; ++q) {
+        uint8_t* dst = static_cast<uint8_t*>(p.g.out_peer[q]) + row_off + n;
+        dst[0] = q0;
+        if (two) dst[1] = q1;
+      }
       return;
     }
-    const uint32_t sc_addr = smem_u32(&ec->sc[buf][col0]), bi_addr = smem_u32(&ec->bi[buf][col0]);
-    const bool hs = p.scales != nullptr, hb = p.bias != nullptr;
-    if (p.out_dt == DT_BF16)
-      epilogue_chunk_fast<__nv_bfloat16, IS_INT>(v, sc_addr, bi_addr, hs, hb,
-                                                 static_cast<__nv_bfloat16*>(out) + row_off + n_first);
-    else if (p.out_dt == DT_F16)
-      epilogue_chunk_fast<__half, IS_INT>(v, sc_addr, bi_addr, hs, hb, static_cast<__half*>(out) + row_off + n_first);
-    else
-      epilogue_chunk_fast<float, IS_INT>(v, sc_addr, bi_addr, hs, hb, static_cast<float*>(out) + row_off + n_first);
-    return;
   }
-  if (p.out_dt == DT_BF16) {
-    epilogue_store16<__nv_bfloat16, IS_INT>(v, static_cast<__nv_bfloat16*>(out) + row_off, n_first, n_limit, true,
-                                           static_cast<const __nv_bfloat16*>(p.scales),
-                                           static_cast<const __nv_bfloat16*>(p.bias), false);
-  } else if (p.out_dt == DT_F16) {
-    epilogue_store16<__half, IS_INT>(v, static_cast<__half*>(out) + row_off, n_first, n_limit, true,
-                                     static_cast<const __half*>(p.scales), static_cast<const __half*>(p.bias), false);
-  } else {
-    epilogue_store16<float, IS_INT>(v, static_cast<float*>(out) + row_off, n_first, n_limit, true,
-                                    static_cast<const float*>(p.scales), static_cast<const float*>(p.bias), false);
-  }
+  const bool vec = ((row_off + n) * sizeof(OT)) % (2 * sizeof(OT)) == 0;
+  for (int q = 0; q < p.g.n_out; ++q) store_pair<OT>(static_cast<OT*>(p.g.out_peer[q]) + row_off + n, f0, f1, two, vec);
 }
 
-template <bool IS_INT, bool ALLOW_Q = false>
-__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32_t (&v)[16], int row, int n_first,
-                                               int n_limit, bool plain, const EpiCols* ec, int buf, int col0) {
-  if (row >= p.M || n_first >= n_limit) return;
-  epilogue_chunk_to<IS_INT, ALLOW_Q>(p, p.out, v, row, n_first, n_limit, plain, ec, buf, col0);
+template <bool ALLOW_Q>
+__device__ __forceinline__ void epilogue_pair(const GemmParams& p, size_t row_off, int n, bool two, float f0, float f1) {
+  if (p.out_dt == DT_BF16) epilogue_pair_t<__nv_bfloat16, ALLOW_Q>(p, row_off, n, two, f0, f1);
+  else if (p.out_dt == DT_F16) epilogue_pair_t<__half, ALLOW_Q>(p, row_off, n, two, f0, f1);
+  else epilogue_pair_t<float, ALLOW_Q>(p, row_off, n, two, f0, f1);
 }
 
 // ------------------------------------------------------------------------------------------------
-// TMA-store epilogue (GemmCfg::EPI == 1)
+// The kernel
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t smem_src, int32_t c0, int32_t c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(map)),
-               "r"(smem_src), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_group_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void bulk_wait_group_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-// 16 fp32 accumulator columns of one row -> 8 registers of OT pairs: rnd(acc), then (bias) rnd(rnd(acc) + bias)
-template <typename OT>
-__device__ __forceinline__ void convert16(const uint32_t* v, bool has_bias, uint32_t bi_addr, uint32_t (&o)[8]) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) o[j] = pack2<OT>(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
-  if (has_bias) {
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const uint4 bv = ld_shared_v4(bi_addr + q * 16);
-      const float2 a = unpack2<OT>(o[2 * q]), b = unpack2<OT>(o[2 * q + 1]);
-      o[2 * q] = pack2<OT>(__fadd_rn(a.x, __uint_as_float(bv.x)), __fadd_rn(a.y, __uint_as_float(bv.y)));
-      o[2 * q + 1] = pack2<OT>(__fadd_rn(b.x, __uint_as_float(bv.z)), __fadd_rn(b.y, __uint_as_float(bv.w)));
-    }
-  }
-}
-
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
-      "%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-
 template <class Cfg>
 __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
     gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                   const __grid_constant__ StoreMaps smaps, const GemmParams p, const uint32_t idesc) {
+                   const GemmParams p) {
   constexpr int NSTAGES = Cfg::NSTAGES;
-  constexpr int MSUB = Cfg::MSUB;
   constexpr int BN = Cfg::BN;
 
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw;
-  if ((smem_u32(smem) & 1023u) != 0u) __trap();  // the swizzled operand tiles need 1024-byte alignment
-  uint8_t* epi_stage = smem + NSTAGES * Cfg::STAGE;  // EPI = 1: [4 warps][2][32 rows x 128 B]
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_stage + Cfg::EPI_STAGE_BYTES);
+  extern __shared__ uint8_t smem_raw[];
+  // the swizzled operand tiles need 1024-byte aligned bases (SMEM_BYTES reserves the slack)
+  const uint32_t raw_addr = smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + NSTAGES * Cfg::STAGE);
   uint64_t* empty_bar = full_bar + NSTAGES;
-  uint64_t* tmem_full_bar = empty_bar + NSTAGES;
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-  EpiCols* epi_cols = reinterpret_cast<EpiCols*>(tmem_ptr_smem + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == Cfg::PRODUCER_WARP * 32) {
     tma_prefetch_desc(&tmap_a);
     if constexpr (Cfg::BSRC == BSrc::TMA) tma_prefetch_desc(&tmap_b);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < NSTAGES; ++s) {
       mbar_init(&full_bar[s], Cfg::FULL_ARRIVALS);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full_bar[a], 1);
-      mbar_init(&tmem_empty_bar[a], 4);
+      mbar_init(&empty_bar[s], Cfg::MWG);  // one arrive per consumer warpgroup
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(tmem_ptr_smem, Cfg::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   const int num_tiles = p.num_m_blocks * p.num_n_blocks;
-  constexpr int A_ELEM = (Cfg::KIND == MmaKind::F16) ? 2 : 1;
+  constexpr int A_ELEM = (Cfg::KIND == MmaKind::F16 || Cfg::KIND == MmaKind::BF16) ? 2 : 1;
   constexpr int KELEMS = Cfg::KBYTES / A_ELEM;  // K elements per stage
   const int kblocks = (p.K + KELEMS - 1) / KELEMS;
+  const uint32_t smem_base = smem_u32(smem);
+  auto a_addr = [&](int s) { return smem_base + s * Cfg::STAGE; };
+  auto b_addr = [&](int s) { return smem_base + s * Cfg::STAGE + Cfg::A_TILE; };
 
-  auto a_smem = [&](int s, int ms) { return smem + s * Cfg::STAGE + ms * Cfg::A_TILE; };
-  auto b_smem = [&](int s) { return smem + s * Cfg::STAGE + MSUB * Cfg::A_TILE; };
-
-  if (warp == 0) {
+  if (warp < Cfg::PRODUCER_WARP) {
+    // ------------------------------------------------------------------ consumers: wgmma + epilogue
+    const int wg = warp >> 2;
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    using AccT = typename std::conditional<Cfg::IS_INT, uint32_t, float>::type;
+    AccT acc[Cfg::NACC];
+    int stage = 0;
+    uint32_t phase = 0;
+    const int half_n = p.N / 2;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int m_blk = tile % p.num_m_blocks;
+      const int n_blk = tile / p.num_m_blocks;
+      int prev = -1;
+      for (int kb = 0; kb < kblocks; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t aa = a_addr(stage) + wg * 64 * Cfg::KBYTES, bb = b_addr(stage);
+        {
+          wgmma_fence();
+          wgmma_slab<Cfg::KIND, BN>(acc, aa, bb, kb > 0);
+          wgmma_commit();
+          // keep one stage of MMAs in flight; the stage before it has been read and goes back to the producers
+          wgmma_wait<1>();
+          wgmma_fence_operands(acc);
+          if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
+          prev = stage;
+        }
+        if (++stage == NSTAGES) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_operands(acc);
+      if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
+      // epilogue straight from the fragment: thread holds rows r0 and r0 + 8, column pairs 8 j + 2 (lane % 4)
+      const int r0 = m_blk * Cfg::BM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = r0 + 8 * h;
+        if (row >= p.M) continue;
+        const size_t row_off = static_cast<size_t>(row) * p.ld + p.col0;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = 8 * j + 2 * (lane & 3);
+          // tile column -> output feature.  int4: columns [0, BN/2) are the low-nibble rows, [BN/2, BN) the high-nibble
+          // rows (+N/2)
+          int n, n_limit;
+          if constexpr (Cfg::BSRC == BSrc::INT4) {
+            if (c < BN / 2) { n = n_blk * (BN / 2) + c; n_limit = half_n; }
+            else { n = half_n + n_blk * (BN / 2) + (c - BN / 2); n_limit = p.N; }
+          } else {
+            n = n_blk * BN + c;
+            n_limit = p.N;
+          }
+          if (n >= n_limit) continue;
+          float f0, f1;
+          if constexpr (Cfg::IS_INT) {
+            f0 = __int2float_rn(static_cast<int>(acc[4 * j + 2 * h]));
+            f1 = __int2float_rn(static_cast<int>(acc[4 * j + 2 * h + 1]));
+          } else {
+            f0 = acc[4 * j + 2 * h];
+            f1 = acc[4 * j + 2 * h + 1];
+          }
+          epilogue_pair<Cfg::BSRC == BSrc::TMA || Cfg::BSRC == BSrc::F8>(p, row_off, n, n + 1 < n_limit, f0, f1);
+        }
+      }
+    }
+    if (p.g.n_out > 1) __threadfence_system();  // this thread's peer stores are performed before the rank signals
+  } else if (warp == Cfg::PRODUCER_WARP) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    if (lane == 0 && Cfg::BSRC != BSrc::F8) {
       int stage = 0;
       uint32_t phase = 0;
-      int tn = 0;
-      constexpr uint32_t tx_bytes = MSUB * Cfg::A_TILE + (Cfg::BSRC == BSrc::TMA ? Cfg::B_TILE : 0);
+      constexpr uint32_t tx_bytes = Cfg::A_TILE + (Cfg::BSRC == BSrc::TMA ? Cfg::B_TILE : 0);
       gather_wait_start(p.g);  // the activation may be the gathered output of the previous linear
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m_blk = tile % p.num_m_blocks;
         const int n_blk = tile / p.num_m_blocks;
         for (int kb = 0; kb < kblocks; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1u);
-          gemm_trace_evt(p, 0, tn);
           mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
-#pragma unroll
-          for (int ms = 0; ms < MSUB; ++ms)
-            tma_load_2d(a_smem(stage, ms), &tmap_a, &full_bar[stage], kb * KELEMS, (m_blk * MSUB + ms) * Cfg::BM);
+          tma_load_2d(smem + stage * Cfg::STAGE, &tmap_a, &full_bar[stage], kb * KELEMS, m_blk * Cfg::BM);
           if constexpr (Cfg::BSRC == BSrc::TMA)
-            tma_load_2d(b_smem(stage), &tmap_b, &full_bar[stage], kb * KELEMS, n_blk * BN);
+            tma_load_2d(smem + stage * Cfg::STAGE + Cfg::A_TILE, &tmap_b, &full_bar[stage], kb * KELEMS, n_blk * BN);
           if (++stage == NSTAGES) { stage = 0; phase ^= 1u; }
         }
       }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (single thread)
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t acc_it = 0;
-      int tn = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++acc_it) {
-        const uint32_t acc = acc_it % Cfg::NACC;
-        const uint32_t acc_phase = (acc_it / Cfg::NACC) & 1u;
-        mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1u);
-        tc_fence_after();
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          gemm_trace_evt(p, 2, tn);
-          const uint32_t b_addr = smem_u32(b_smem(stage));
-#pragma unroll
-          for (int k = 0; k < Cfg::KBYTES / 32; ++k) {
-            const uint64_t b_desc = umma_desc_sw128_kmajor(b_addr + k * 32);
-#pragma unroll
-            for (int ms = 0; ms < MSUB; ++ms) {
-              const uint64_t a_desc = umma_desc_sw128_kmajor(smem_u32(a_smem(stage, ms)) + k * 32);
-              tc_mma<Cfg::KIND>(tmem_base + acc * Cfg::ACC_COLS + ms * BN, a_desc, b_desc, idesc,
-                                (kb | k) != 0 ? 1u : 0u);
-            }
-          }
-          tc_commit(&empty_bar[stage]);  // smem slot reusable once these MMAs have read it
-          if (++stage == NSTAGES) { stage = 0; phase ^= 1u; }
-        }
-        tc_commit(&tmem_full_bar[acc]);  // accumulator complete -> epilogue
-      }
-    }
-  } else if (warp < 6) {
-    // ------------------------------------------------------------------ epilogue (4 warps = 128 TMEM lanes)
-    const int quarter = warp & 3;
-    uint32_t acc_it = 0;
-    int epi_grp = 0;  // EPI = 1: running count of staged blocks (selects the staging buffer)
-    const bool int_split = (Cfg::BSRC == BSrc::INT4);
-    const int half_n = p.N / 2;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++acc_it) {
-      const int m_blk = tile % p.num_m_blocks;
-      const int n_blk = tile / p.num_m_blocks;
-      const uint32_t acc = acc_it % Cfg::NACC;
-      const uint32_t acc_phase = (acc_it / Cfg::NACC) & 1u;
-      // All MSUB * BN / 16 chunks of the tile as one software-pipelined sequence: the TMEM load of chunk c+1 is in
-      // flight while chunk c is converted and stored.
-      constexpr int NCH = MSUB * (BN / 16);
-      constexpr bool IS_INT = (Cfg::KIND == MmaKind::I8);
-      const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * Cfg::ACC_COLS;
-      const bool plain = (p.scales == nullptr) && (p.bias == nullptr) && !IS_INT;
-      // tile column -> output feature.  int4: columns [0, BN/2) are the low-nibble rows, [BN/2, BN) the high-nibble
-      // rows (+N/2)
-      auto col_first = [&](int c, int& n_limit) {
-        if (int_split) {
-          if (c < BN / 2) { n_limit = half_n; return n_blk * (BN / 2) + c; }
-          n_limit = p.N;
-          return half_n + n_blk * (BN / 2) + (c - BN / 2);
-        }
-        n_limit = p.N;
-        return n_blk * BN + c;
-      };
-      const int buf = static_cast<int>(acc_it & 1u);
-      if constexpr (Cfg::EPI == 1) {
-        // ---- staged TMA-store epilogue (fp16 / bf16 outputs, no per-column scale: the int4 and weight-only kernels)
-        using OT = typename Cfg::WT;
-        float* bias_s = reinterpret_cast<float*>(epi_cols) + buf * 256;
-        const bool has_bias = p.bias != nullptr;
-        if (has_bias) {
-          for (int c = threadIdx.x - 64; c < BN; c += 128) {
-            int lim;
-            const int n = col_first(c, lim);
-            bias_s[c] = (n < lim) ? load_out_dt_as_float(p.bias, p.out_dt, n) : 0.f;
-          }
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-        }
-        mbar_wait(&tmem_full_bar[acc], acc_phase);
-        tc_fence_after();
-        const uint32_t sbuf0 = smem_u32(epi_stage) + static_cast<uint32_t>(quarter) * 8192u;
-        const uint32_t my_row = static_cast<uint32_t>(lane) * 128u, sw = static_cast<uint32_t>(lane) & 7u;
-        constexpr int NGRP = MSUB * (BN / 64);
-#pragma unroll 1
-        for (int grp = 0; grp < NGRP; ++grp) {
-          const int ms = grp / (BN / 64), cg = grp % (BN / 64);
-          const uint32_t sbuf = sbuf0 + static_cast<uint32_t>((epi_grp + grp) & 1) * 4096u;
-          uint32_t v0[32], v1[32];
-          tmem_ld_32x32b_x32(t_lane + ms * BN + cg * 64, v0);
-          tmem_ld_32x32b_x32(t_lane + ms * BN + cg * 64 + 32, v1);
-          if (lane == 0) bulk_wait_group_read<1>();  // the store that last read this buffer has consumed it
-          __syncwarp();
-          tmem_ld_wait();
-#pragma unroll
-          for (int h = 0; h < 4; ++h) {
-            uint32_t o[8];
-            convert16<OT>(h < 2 ? &v0[16 * h] : &v1[16 * (h - 2)], has_bias,
-                          smem_u32(bias_s + cg * 64 + h * 16), o);
-            st_shared_v4(sbuf + my_row + (((2u * h) ^ sw) << 4), o[0], o[1], o[2], o[3]);
-            st_shared_v4(sbuf + my_row + (((2u * h + 1u) ^ sw) << 4), o[4], o[5], o[6], o[7]);
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            int n_limit;
-            const int n_first = col_first(cg * 64, n_limit);
-            const int row0 = (m_blk * MSUB + ms) * Cfg::BM + quarter * 32;
-            if (n_first < n_limit && row0 < p.M) {
-#pragma unroll 1
-              for (int q = 0; q < p.g.n_out; ++q) tma_store_2d(&smaps.m[q], sbuf, p.col0 + n_first, row0);
-            }
-            bulk_commit_group();
-          }
-        }
-        epi_grp += NGRP;
-      } else {
-      if (!plain) {
-        epi_stage_cols(epi_cols, buf, p, threadIdx.x - 64, BN, [&](int c) {
-          int lim;
-          const int n = col_first(c, lim);
-          return n < lim ? n : -1;
-        });
-      }
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tc_fence_after();
-      uint32_t va[16], vb[16];
-      tmem_ld_32x32b_x16(t_lane, va);
-      tmem_ld_wait();
-      auto do_chunk = [&](int ch, const uint32_t (&v)[16]) {
-        const int ms = ch / (BN / 16), chunk = ch % (BN / 16);
-        const int row = (m_blk * MSUB + ms) * Cfg::BM + quarter * 32 + lane;
-        int n_limit;
-        const int n_first = col_first(chunk * 16, n_limit);
-        epilogue_chunk<IS_INT, (Cfg::KIND != MmaKind::F16)>(p, v, row, n_first, n_limit, plain, epi_cols, buf,
-                                                                        chunk * 16);
-      };
-#pragma unroll 1
-      for (int ch = 0; ch < NCH; ch += 2) {
-        tmem_ld_32x32b_x16(t_lane + (ch + 1) * 16, vb);  // NCH is even
-        do_chunk(ch, va);
-        tmem_ld_wait();
-        if (ch + 2 < NCH) tmem_ld_32x32b_x16(t_lane + (ch + 2) * 16, va);
-        do_chunk(ch + 1, vb);
-        tmem_ld_wait();
-      }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty_bar[acc]);
-    }
-    if constexpr (Cfg::EPI == 1) {
-      if (lane == 0) bulk_wait_group_all();  // every output store of this warp has been performed
-      (void)epi_grp;
     }
   } else {
-    // ------------------------------------------------------------------ weight staging (int4 -> WT tile)
+    // ------------------------------------------------------------------ weight staging (int4 / 8-bit -> WT tile)
+    const int ct = threadIdx.x - Cfg::FIRST_CVT_WARP * 32;
+    constexpr int GT = Cfg::CVT_GROUP_WARPS * 32;  // threads per staging group
+    const int grp = ct / GT;                         // staging group == pipeline slot it owns
+    const int r = ct % GT;
+    const int my_tiles = (num_tiles > static_cast<int>(blockIdx.x))
+                             ? (num_tiles - 1 - static_cast<int>(blockIdx.x)) / static_cast<int>(gridDim.x) + 1
+                             : 0;
+    const int total_it = my_tiles * kblocks;
+    const uint32_t bt = b_addr(grp);  // this group's B tile
+    const uint32_t full_addr = smem_u32(full_bar) + grp * 8, empty_addr = smem_u32(empty_bar) + grp * 8;
+    const uint32_t sw = static_cast<uint32_t>(r) & 7;
     if constexpr (Cfg::BSRC == BSrc::INT4) {
       using WT = typename Cfg::WT;
       using D = Dq<WT>;
       constexpr bool ZP = Cfg::ZP;
-      constexpr int ROWP = BN / 2;  // packed rows per tile
-      constexpr int GT = Cfg::CVT_GROUP_WARPS * 32;  // threads per staging group (>= ROWP; extra lanes only synchronise)
-      static_assert(ROWP % 8 == 0, "both rows of a pair must share the swizzle phase");
-      const int ct = threadIdx.x - 6 * 32;
-      const int grp = ct / GT;      // staging group == pipeline slot it owns
-      const int r = ct % GT;        // packed row inside the tile
-      const bool active = r < ROWP;
+      constexpr int ROWP = BN / 2;  // packed rows per tile, one per thread of the group
+      static_assert(ROWP == GT, "one staging thread per packed row");
       const int half_n = p.N / 2;
       const int groups_per_row = p.K / p.group;
       const bool two_sets = p.group < 64;  // group size 32: two (scale, shift) pairs per 64-k stage
       const WT* scale = static_cast<const WT*>(p.wscale);
-
-      const int my_tiles = (num_tiles > static_cast<int>(blockIdx.x))
-                               ? (num_tiles - 1 - static_cast<int>(blockIdx.x)) / static_cast<int>(gridDim.x) + 1
-                               : 0;
-      const int total_it = my_tiles * kblocks;
 
       // This group's stage sequence: it = grp, grp + NSTAGES, ...   (tile, kb) advance incrementally.
       struct Pre {
@@ -917,7 +561,7 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
         if (f_it >= total_it) return;
         const int rp = (f_tile / p.num_m_blocks) * ROWP + r;
         const int kbase = f_kb * 64;
-        pr.ok = active && rp < half_n && kbase < p.K;
+        pr.ok = rp < half_n && kbase < p.K;
         if (pr.ok) {
           const uint8_t* src = p.wq + static_cast<size_t>(rp) * p.K + kbase;
 #pragma unroll
@@ -930,7 +574,7 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
             if (st == 1 && kbase + 32 >= p.K) {
               // K tail (K % 64 == 32 with groups of 32): the second half of the stage lies beyond K -- its activations are
               // zero-filled, but its coefficients would be read past the row (past the ARRAY for the last row: NaN bits
-              // there turn 0 * w into NaN; found by the reference's nn/test_qlinear.py at K = 32)
+              // there turn 0 * w into NaN)
               pr.s_lo[1] = pr.s_lo[0]; pr.s_hi[1] = pr.s_hi[0]; pr.z_lo[1] = pr.z_lo[0]; pr.z_hi[1] = pr.z_hi[0];
               break;
             }
@@ -952,19 +596,11 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
         while (f_kb >= kblocks) { f_kb -= kblocks; f_tile += gridDim.x; }
       };
 
-      const uint32_t sw = static_cast<uint32_t>(r) & 7;
       const uint32_t off_lo = (static_cast<uint32_t>(r) >> 3) * 1024 + (static_cast<uint32_t>(r) & 7) * 128;
       const uint32_t off_hi = off_lo + (ROWP / 8) * 1024;
-      const uint32_t bt = smem_u32(smem) + grp * Cfg::STAGE + MSUB * Cfg::A_TILE;  // this group's B tile
-      const uint32_t full_addr = smem_u32(full_bar) + grp * 8, empty_addr = smem_u32(empty_bar) + grp * 8;
-
       uint32_t phase = 0;
-      int tn = 0;
-      const bool tracer = (ct == 0);
       auto process = [&](const Pre& cur) {
-        if (tracer) gemm_trace_evt(p, 4, tn);
         mbar_wait_u32(empty_addr, phase ^ 1u);
-        if (tracer) gemm_trace_evt(p, 4, tn);
         if (cur.ok) {
           typename D::Coef klo[2], khi[2];
           klo[0] = D::make_raw(cur.s_lo[0], cur.z_lo[0], ZP);
@@ -977,14 +613,12 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
             khi[1] = khi[0];
           }
           stage_rowpair_64k<WT, ZP>(cur.raw, klo, khi, bt + off_lo, bt + off_hi, sw);
-        } else if (active) {
+        } else {
           zero_rowpair_64k(bt + off_lo, bt + off_hi);
         }
-        if (tracer) gemm_trace_evt(p, 4, tn);
         fence_proxy_async_smem();  // every writer: generic-proxy stores -> visible to the async proxy
-        if (tracer) gemm_trace_evt(p, 4, tn);
         __syncwarp();
-        if (lane == 0) mbar_arrive_u32(full_addr);  // one arrive per warp (per-thread arrives serialise)
+        if (lane == 0) mbar_arrive_u32(full_addr);  // one arrive per warp
         phase ^= 1u;
       };
       // Ping-pong prefetch buffers (no register copies: copying a register that a load is still filling would
@@ -1000,19 +634,12 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
         }
       }
     }
-    if constexpr (Cfg::BSRC == BSrc::BYTES) {
-      // ---------------- 8-bit weights (int8 / fp8) -> activation dtype, scale pre-applied (reference rounding order)
+    if constexpr (Cfg::BSRC == BSrc::BYTES || Cfg::BSRC == BSrc::F8) {
+      // ---------------- 8-bit weights (int8 / fp8) -> activation dtype, scale pre-applied (reference rounding order);
+      // F8: the weights unscaled (the scale is applied to the fp32 result) and the activation rows of the tile as well
       using WT = typename Cfg::WT;
-      constexpr int GT = BN / 2;  // threads per staging group; thread r converts weight rows r and r + BN/2
-      static_assert(GT % 32 == 0, "8-bit staging groups are whole warps");
-      const int ct = threadIdx.x - 6 * 32;
-      const int grp = ct / GT;
-      const int r = ct % GT;
+      static_assert(GT == BN / 2, "thread r converts weight rows r and r + BN/2");
       const WT* scale = static_cast<const WT*>(p.wscale);
-      const int my_tiles = (num_tiles > static_cast<int>(blockIdx.x))
-                               ? (num_tiles - 1 - static_cast<int>(blockIdx.x)) / static_cast<int>(gridDim.x) + 1
-                               : 0;
-      const int total_it = my_tiles * kblocks;
       struct PreB {
         uint4 raw0[4], raw1[4];
       };
@@ -1036,16 +663,15 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
         f_kb += NSTAGES;
         while (f_kb >= kblocks) { f_kb -= kblocks; f_tile += gridDim.x; }
       };
-      const uint32_t sw = static_cast<uint32_t>(r) & 7;
       const uint32_t off0 = (static_cast<uint32_t>(r) >> 3) * 1024 + (static_cast<uint32_t>(r) & 7) * 128;
       const uint32_t off1 = off0 + (GT / 8) * 1024;
-      const uint32_t bt = smem_u32(smem) + grp * Cfg::STAGE + MSUB * Cfg::A_TILE;
-      const uint32_t full_addr = smem_u32(full_bar) + grp * 8, empty_addr = smem_u32(empty_bar) + grp * 8;
       uint32_t phase = 0;
       int c_tile = -1, c_kb = grp % kblocks, c_t = blockIdx.x + (grp / kblocks) * gridDim.x;
       uint32_t s2_0 = 0, s2_1 = 0;
       auto process = [&](const PreB& cur) {
-        if (c_t != c_tile) {  // new tile: (re)load the two per-row scales (zero rows beyond N contribute exact zeros)
+        if (Cfg::BSRC == BSrc::F8) {
+          s2_0 = s2_1 = 0x3F803F80u;  // bf16 1.0 pair: the conversion alone, exact
+        } else if (c_t != c_tile) {  // new tile: (re)load the two per-row scales (zero rows beyond N contribute exact zeros)
           c_tile = c_t;
           const int n0 = (c_t / p.num_m_blocks) * BN + r;
           const int n1 = n0 + GT;
@@ -1058,6 +684,25 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
         mbar_wait_u32(empty_addr, phase ^ 1u);
         stage_row_64k<WT, Cfg::WKIND>(cur.raw0, s2_0, bt + off0, sw);
         stage_row_64k<WT, Cfg::WKIND>(cur.raw1, s2_1, bt + off1, sw);
+        if constexpr (Cfg::BSRC == BSrc::F8) {
+          // activation rows r and r + 64 of the tile (BM = 64 or 128), loaded here rather than prefetched: the staging
+          // thread has no registers left for a second pair of ping-pong buffers
+          const int kbase = c_kb * 64;
+          const uint32_t at = bt - Cfg::A_TILE;
+#pragma unroll
+          for (int h = 0; h < Cfg::BM / 64; ++h) {
+            const int ar = r + 64 * h;
+            const int m = (c_t % p.num_m_blocks) * Cfg::BM + ar;
+            uint4 raw[4];
+#pragma unroll
+            for (int v = 0; v < 4; ++v)
+              raw[v] = (m < p.M && kbase + v * 16 < p.K)
+                           ? __ldg(reinterpret_cast<const uint4*>(static_cast<const uint8_t*>(p.a) + static_cast<size_t>(m) * p.K + kbase) + v)
+                           : make_uint4(0, 0, 0, 0);
+            const uint32_t aoff = (static_cast<uint32_t>(ar) >> 3) * 1024 + (static_cast<uint32_t>(ar) & 7) * 128;
+            stage_row_64k<WT, Cfg::AKIND>(raw, 0x3F803F80u, at + aoff, sw);
+          }
+        }
         fence_proxy_async_smem();
         __syncwarp();
         if (lane == 0) mbar_arrive_u32(full_addr);
@@ -1065,26 +710,30 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
         c_kb += NSTAGES;
         while (c_kb >= kblocks) { c_kb -= kblocks; c_t += gridDim.x; }
       };
-      PreB pa, pb;
-      load_pre(pa);
-      for (int it = grp; it < total_it; it += 2 * NSTAGES) {
-        load_pre(pb);
-        process(pa);
-        if (it + NSTAGES < total_it) {
+      if constexpr (Cfg::BSRC == BSrc::F8) {
+        // one stage in registers at a time: the activation rows of the stage need the registers of a second buffer
+        for (int it = grp; it < total_it; it += NSTAGES) {
+          PreB pa;
           load_pre(pa);
-          process(pb);
+          process(pa);
+        }
+      } else {
+        PreB pa, pb;
+        load_pre(pa);
+        for (int it = grp; it < total_it; it += 2 * NSTAGES) {
+          load_pre(pb);
+          process(pa);
+          if (it + NSTAGES < total_it) {
+            load_pre(pa);
+            process(pb);
+          }
         }
       }
     }
   }
 
-  tc_fence_before();
   __syncthreads();
   if (threadIdx.x == 0) gather_signal_end(p.g);  // fused all-gather: publish "this rank's slab has landed everywhere"
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
 }
 
 }  // namespace qb

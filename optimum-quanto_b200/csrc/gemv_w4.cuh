@@ -8,21 +8,48 @@
 // mma.sync.m16n8k16 (16 out-features x 8 tokens per instruction) whose B fragment is the activation vector.
 // The k index of an MMA is only a summation index, so the k positions are permuted to what the loads deliver
 // (thread t of a quad owns k = 16t..16t+15 of each 64-k slab, k-step s uses its bytes 4s..4s+3) and the activation
-// fragment is gathered with the same permutation.  The legacy warp MMA is used on purpose: at <= 32 tokens the math is
-// <2 % of the tensor peak, and unlike tcgen05 it takes its operands from registers, which is where the exact
-// dequantisation leaves them (the tcgen05 variant in gemm_decode.cuh spends more time moving the dequantised tile
-// into TMEM than HBM needs to deliver the packed bytes; it remains the path for 32 < M <= 128).
+// fragment is gathered with the same permutation.  The warp MMA is used on purpose: at <= 32 tokens the math is
+// <2 % of the tensor peak, and unlike wgmma it takes its operands from registers, which is where the exact
+// dequantisation leaves them.
 //
-// Decomposition: identical stream-K scheme and split-K fix-up as gemm_decode.cuh (blocks of 64 packed rows = 128
-// out-features, stages of 128 k, equal contiguous spans per CTA, deterministic ticket reduction), so the workspace
-// contract of qb200_qbits_mm is unchanged.  CTA = 8 warps: warp w handles the 16 packed rows (w & 3) of the block and
-// the 64-k half (w >> 2) of every stage.
+// Decomposition (stream-K): blocks of 64 packed rows = 128 out-features, stages of 128 k; the P*K/128 stages are dealt
+// to the CTAs in equal contiguous spans, so every SM streams the same number of bytes whatever N is.  A span is cut
+// into segments at block boundaries; a block finished by several CTAs is reduced deterministically: every segment
+// writes its fp32 partial to the workspace, an atomic ticket per block elects the last arriver, which sums the
+// partials in segment order, rounds once, adds the bias and stores.  CTA = 8 warps: warp w handles the 16 packed rows
+// (w & 3) of the block and the 64-k half (w >> 2) of every stage.
 #pragma once
 
 #include "common.cuh"
-#include "gemm_decode.cuh"
+#include "gather.cuh"
+#include "gemm_tc.cuh"
 
 namespace qb {
+
+struct DecodeParams {
+  const void* scale;   // [N * K / group] weight dtype
+  const void* shift;   // same, or uint8 zero-points
+  const void* bias;    // [N] or nullptr
+  void* out;           // [M, ld] (ld = N, col0 = 0 for an ordinary call)
+  GatherInfo g;        // fused all-gather of a column-parallel linear (gather.cuh); g.n_out == 1: ordinary call
+  int ld, col0;
+  float* partials;     // workspace: [P][max_segs][M][128] fp32
+  int* tickets;        // workspace: [P] zero-initialised once; the kernel leaves them zero
+  int M, N, K;
+  int group;
+  int group_log2;      // log2(group) or -1
+  int shift_is_int;
+  int P;               // out-feature blocks = ceil((N/2) / 64)
+  int SPB;             // 128-k stages per block = K / 128
+  int span;            // stages per CTA
+  int max_segs;
+  int dbg;             // developer knock-out flags (KNOCKOUTS=1 builds only)
+};
+
+// number of segments block `pb` is cut into when spans have `span` stages
+__device__ __forceinline__ int decode_nsegs(int pb, int spb, int span) {
+  return ((pb + 1) * spb - 1) / span - (pb * spb) / span + 1;
+}
 
 template <typename WT>
 __device__ __forceinline__ void mma_m16n8k16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1);

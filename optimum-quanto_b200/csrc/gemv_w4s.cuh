@@ -5,7 +5,7 @@
 //   * every CTA owns a contiguous range of PACKED rows (= out-feature pairs n, n + N/2) over the whole K, so there is
 //     no split-K, no workspace, no tickets and the result is deterministic by construction;
 //   * one elected thread streams those rows with cp.async.bulk (TMA, 1-D) into a ring that holds ~190 KB per SM --
-//     148 SMs x 190 KB is the whole matrix in flight at launch, HBM never waits for an instruction to be issued;
+//     132 SMs x 190 KB is the whole matrix in flight at launch, HBM never waits for an instruction to be issued;
 //   * 16 compute warps read the ring with conflict-free LDS.128 (rows padded by 64 B), dequantise in registers with the
 //     reference's rounding order (tensor/qbits.py:34-45) and accumulate with mma.sync.m16n8k16: MMA rows 0-7 are the
 //     low nibbles of 8 packed rows, rows 8-15 their high nibbles, the 8 MMA columns are the (<= 8) tokens;

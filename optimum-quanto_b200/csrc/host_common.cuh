@@ -21,7 +21,7 @@ void set_kernel_family(int family);
 constexpr int kMaxDevices = 64;
 int current_device();       // cudaGetDevice, -1 on error
 int current_sm_count();     // multiprocessors of the current device
-int check_arch();           // OK when the current device is sm_100, else ERR_ARCH (message set)
+int check_arch();           // OK when the current device is sm_90 (Hopper), else ERR_ARCH (message set)
 
 // Opt the kernel into `bytes` of dynamic shared memory on the current device (once per kernel and device).  The kernel
 // is a template ARGUMENT: one static per kernel function (kernels of different configurations share a pointer TYPE).
@@ -66,14 +66,14 @@ int make_tmap_2d_view(CUtensorMap* map, const void* base, int dt, int64_t rows, 
 
 // ---- test hooks (include/quanto_b200.h: qb200_test_override).  Every value selects a kernel that computes the same
 // result; 0 = automatic choice.  They exist so that the test-suite can execute every shipped instantiation.
-enum : int { OVR_INT4_TILE_N = 0, OVR_QBYTES_TILE_N = 1, OVR_INT4_ROUTE = 2, OVR_QBYTES_ROUTE = 3, OVR_EPILOGUE = 4,
-             OVR_GEMV_PRODUCER = 5, OVR_PDL = 6 /* 1 = no programmatic dependent launch */,
-             OVR_GEMV_SHAPE = 7 /* 2 = the two-CTAs-per-SM shape of the ring gemv (M <= 2) */, OVR_COUNT = 8 };
+enum : int { OVR_TILE_M = 0 /* 64 | 128 rows per wgmma tile */, OVR_QBYTES_TILE_N = 1 /* int8: 128 | 256 */,
+             OVR_INT4_ROUTE = 2, OVR_QBYTES_ROUTE = 3, OVR_GEMV_PRODUCER = 4,
+             OVR_PDL = 5 /* 1 = no programmatic dependent launch */,
+             OVR_GEMV_SHAPE = 6 /* 2 = the two-CTAs-per-SM shape of the ring gemv (M <= 2) */, OVR_COUNT = 7 };
 // OVR_INT4_ROUTE values
-enum : int { ROUTE_AUTO = 0, ROUTE_INT4_GENERAL = 1, ROUTE_INT4_TCDECODE = 2, ROUTE_INT4_GEMV = 3, ROUTE_INT4_RING = 4,
-             ROUTE_INT4_PAIR = 5, ROUTE_INT4_PAIR_TMEM = 6, ROUTE_INT4_SINGLE = 7, ROUTE_INT4_RING2 = 8 };
+enum : int { ROUTE_AUTO = 0, ROUTE_INT4_GENERAL = 1, ROUTE_INT4_GEMV = 3, ROUTE_INT4_RING = 4, ROUTE_INT4_RING2 = 8 };
 // OVR_QBYTES_ROUTE values
-enum : int { ROUTE_QBYTES_SINGLE = 1, ROUTE_QBYTES_SIMT = 2 };
+enum : int { ROUTE_QBYTES_SIMT = 2 };
 int test_override(int key);
 
 // ---- developer knock-outs: only a KNOCKOUTS=1 build honours them; a release build reports and uses 0

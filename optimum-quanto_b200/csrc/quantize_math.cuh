@@ -64,7 +64,7 @@ __device__ __forceinline__ uint8_t quantize_one(float t) {
     float c = fminf(fmaxf(t, -448.f), 448.f);
     return static_cast<uint8_t>(__nv_cvt_float_to_fp8(c, __NV_SATFINITE, __NV_E4M3));
   } else if constexpr (OUT_DT == DT_E4M3FNUZ) {
-    // float8_e4m3fnuz (optimum/quanto/tensor/qtype.py:63): no native convert on sm_100.  Round-half-even to 3 mantissa
+    // float8_e4m3fnuz (optimum/quanto/tensor/qtype.py:63): no native convert.  Round-half-even to 3 mantissa
     // bits on the fp32 pattern (normals) / to a multiple of 2^-10 (subnormals); zero has no sign, NaN is 0x80.
     if (t != t) return 0x80u;
     const float c = fminf(fmaxf(t, -240.f), 240.f);

@@ -1,4 +1,4 @@
-"""quanto_b200 -- B200-native (sm_100a) kernels behind optimum-quanto's quantized-linear operator surface.
+"""quanto_b200 -- H100-native (sm_90a) kernels behind optimum-quanto's quantized-linear operator surface.
 
 Importing the package registers the `torch.ops.quanto.*` CUDA implementations (library.py) and exposes the host-side
 mirror of the reference classes on the hot path.  The native library is loaded lazily at the first op call and

@@ -1,11 +1,11 @@
-"""Bind the sm_100a kernels into the REAL `optimum.quanto` package (the binding INTEGRATION.md describes, executable).
+"""Bind the sm_90a kernels into the REAL `optimum.quanto` package (the binding INTEGRATION.md describes, executable).
 
     import optimum.quanto                      # the reference, unmodified
     from quanto_b200.integration import bind_reference
     bind_reference()
 
 After this, every `optimum.quanto` object keeps working as before -- `quantize()`, `freeze()`, `QLinear`,
-`WeightQBitsTensor`, state dicts -- and the quantized-linear forward on a CUDA (sm_100) device runs on this library:
+`WeightQBitsTensor`, state dicts -- and the quantized-linear forward on a CUDA (sm_90) device runs on this library:
 
 1. op registry: `quanto::unpack`, `quanto::quantize_symmetric`, `quanto::qbytes_mm` (and `quanto::quantize_affine`) get
    this library's CUDA implementations (importing `quanto_b200.library` after the reference re-binds the CUDA dispatch key;

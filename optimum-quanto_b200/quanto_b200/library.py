@@ -1,4 +1,4 @@
-"""`torch.ops.quanto.*` registry backed by the sm_100a kernels (C-ABI in include/quanto_b200.h).
+"""`torch.ops.quanto.*` registry backed by the sm_90a kernels (C-ABI in include/quanto_b200.h).
 
 Keeps the reference's op names and schemas so that QTensor code written against quanto keeps working:
   quanto::unpack             optimum/quanto/library/unpack.py:18
@@ -115,7 +115,7 @@ def quantize_symmetric_cuda(base: torch.Tensor, dtype: torch.dtype, axis: Option
     if base.dtype not in (torch.float32, torch.float16, torch.bfloat16):
         raise ValueError(f"quantize_symmetric: unsupported base dtype {base.dtype}")
     if dtype not in (torch.int8, torch.float8_e4m3fn, torch.float8_e5m2, torch.float8_e4m3fnuz):
-        raise NotImplementedError(f"quantize_symmetric: no sm_100a kernel for target dtype {dtype}")
+        raise NotImplementedError(f"quantize_symmetric: no sm_90a kernel for target dtype {dtype}")
     base = _require_contiguous(base, "base")
     scale = scale.to(base.dtype)
     if axis is None:
@@ -263,7 +263,7 @@ def quantize_qbytes_absmax_cuda(base: torch.Tensor, dtype: torch.dtype):
     if base.dtype not in _FLOATS:
         raise ValueError(f"quantize_qbytes_absmax: unsupported dtype {base.dtype}")
     if dtype not in (torch.int8, torch.float8_e4m3fn, torch.float8_e5m2):
-        raise NotImplementedError(f"quantize_qbytes_absmax: no sm_100a kernel for target dtype {dtype}")
+        raise NotImplementedError(f"quantize_qbytes_absmax: no sm_90a kernel for target dtype {dtype}")
     base = _require_contiguous(base, "base")
     n, k = base.shape
     data = torch.empty((n, k), dtype=dtype, device=base.device)
@@ -299,7 +299,7 @@ def qbytes_mm_cuda(activations: torch.Tensor, weights: torch.Tensor, output_scal
     if activations.shape[-1] != k:
         raise ValueError(f"qbytes_mm: in_features mismatch ({activations.shape[-1]} vs {k})")
     if weights.dtype not in (torch.int8, torch.float8_e4m3fn, torch.float8_e5m2, torch.float8_e4m3fnuz):
-        raise NotImplementedError(f"qbytes_mm: no sm_100a kernel for weights of dtype {weights.dtype}")
+        raise NotImplementedError(f"qbytes_mm: no sm_90a kernel for weights of dtype {weights.dtype}")
     if activations.dtype not in N.DTYPE_CODE or activations.dtype == torch.uint8:
         raise NotImplementedError(f"qbytes_mm: unsupported activations dtype {activations.dtype}")
     out_dtype = output_scales.dtype
@@ -438,7 +438,7 @@ def qbits_mm_cuda(activations, packed, scale, shift, bias, out_features: int, gr
 
 
 def _bind_cuda(name: str, fn):
-    """Attach the sm_100a implementation to the CUDA dispatch key, replacing the reference's CUDA binding if
+    """Attach the sm_90a implementation to the CUDA dispatch key, replacing the reference's CUDA binding if
     `optimum.quanto` was imported first (it registers its own for unpack / qbytes_mm,
     optimum/quanto/library/extensions/cuda/__init__.py:77-79, library/qbytes_mm.py:73)."""
     _lib.impl(name, fn, "CUDA", allow_override=True)

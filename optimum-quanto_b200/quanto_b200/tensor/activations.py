@@ -1,6 +1,6 @@
 """Per-tensor 8-bit quantized activations (optimum/quanto/tensor/activations/qbytes.py:28-92, quantization.py:24-39).
 
-Only what the linear hot path needs is kept: construction through `quanto::quantize_symmetric` (one sm_100a kernel),
+Only what the linear hot path needs is kept: construction through `quanto::quantize_symmetric` (one sm_90a kernel),
 flatten/unflatten, and a dequantising fallback for every aten op.  The reference's table of quantized attention ops
 (qbytes_ops.py) is out of scope (SURVEY 2, row 14); `F.linear` never reaches it because the weight's
 `__torch_function__` intercepts first.

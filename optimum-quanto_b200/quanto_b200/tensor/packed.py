@@ -3,7 +3,7 @@
 Storage contract (kept bit-for-bit, it is quanto's on-disk format, optimum/quanto/tensor/packed.py:24-163):
 rows are split into 8/bits planes of R = ceil(rows / (8/bits)) rows; byte (i, c) holds plane p at bits [p*bits, (p+1)*bits).
 For an int4 [N*K/G, G] weight this means: low nibble = out-features [0, N/2), high nibble = [N/2, N), same k.
-`unpack()` goes through `torch.ops.quanto.unpack`, i.e. the sm_100a kernel on CUDA tensors.
+`unpack()` goes through `torch.ops.quanto.unpack`, i.e. the sm_90a kernel on CUDA tensors.
 """
 import ast
 
@@ -18,7 +18,7 @@ def pack_weights(intweights: torch.Tensor, bits: int) -> torch.Tensor:
     if bits not in (2, 4):
         raise ValueError("bits must be 2 or 4")
     if intweights.is_cuda:
-        return torch.ops.quanto.pack(intweights.to(torch.uint8), bits)  # one sm_100a launch (csrc/freeze.cu)
+        return torch.ops.quanto.pack(intweights.to(torch.uint8), bits)  # one sm_90a launch (csrc/freeze.cu)
     # CPU tensors (building / loading a model on the host): the reference's slice-shift-or loop
     per_byte = 8 // bits
     rows = intweights.shape[0]

@@ -3,7 +3,7 @@
 Same constructor signatures, factory names, serialization keys and torch-function/dispatch hooks as
 optimum/quanto/tensor/weights/qbytes.py:31-326 and optimum/quanto/tensor/weights/qbits.py:34-317.  The difference
 is in `create()`: there is no kernel-specific repacking any more (AWQ / Marlin / TinyGemm subclasses are gone); the
-B200 kernels read quanto's canonical storage directly, so `create()` always returns the canonical class and
+The kernels read quanto's canonical storage directly, so `create()` always returns the canonical class and
 `optimize()` is the identity.
 """
 import ast
@@ -40,7 +40,7 @@ class WeightQBytesQuantizer(Function):
 class WeightQBytesTensor(QBytesTensor):
     @staticmethod
     def create(qtype, axis, size, stride, data, scale, activation_qtype: Optional[qtype] = None, requires_grad=False):
-        """Factory kept for API compatibility; the canonical tensor is already the optimal one on B200."""
+        """Factory kept for API compatibility; the canonical tensor is already the optimal one on H100."""
         return WeightQBytesTensor(qtype, axis, size, stride, data, scale, activation_qtype, requires_grad)
 
     @staticmethod
@@ -168,7 +168,7 @@ class WeightsQBitsQuantizer(Function):
 class WeightQBitsTensor(QBitsTensor):
     @staticmethod
     def create(qtype, axis, group_size, size, stride, data, scale, shift, requires_grad=False):
-        """No AWQ / TinyGemm routing: the fused sm_100a kernel consumes the canonical packing as is."""
+        """No AWQ / TinyGemm routing: the fused sm_90a kernel consumes the canonical packing as is."""
         return WeightQBitsTensor(qtype, axis, group_size, size, stride, data, scale, shift, requires_grad)
 
     @staticmethod

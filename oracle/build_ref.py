@@ -4,10 +4,10 @@ TEST / BENCH INFRASTRUCTURE, git-ignored, never imported by the product.  `pip i
 reference (its wheel omits the JIT extension sources, which are overlaid from the same tree), its own tests and bench
 scripts beside it, and its two JIT extensions pre-built here so that the GPU box (same image, no /root/reference, no
 network) can import them without compiling: `quanto_cpp` (CPU unpack) and `quanto_cuda` (unpack, AWQ v2, Marlin int4 /
-fp8 -- the kernels the reference itself would dispatch to on a B200, SURVEY 2.2), cross-compiled for sm_100.
+fp8 -- the kernels the reference itself would dispatch to on an H100, SURVEY 2.2), cross-compiled for sm_90.
 
 Used by: bench.py --impl reference (kind "reference" when importable), tools/run_reference_tests.py (the reference's
-own hot-path tests against the sm_100a ops), tools/compare_reference_kernels.py (same-box kernel comparison).
+own hot-path tests against the sm_90a ops).
 
     python oracle/build_ref.py [--cuda]
 """
@@ -42,7 +42,7 @@ def main():
     torch.ops.quanto.unpack(packed, 4)
     print("quanto_cpp built")
     if "--cuda" in sys.argv:
-        os.environ["TORCH_CUDA_ARCH_LIST"] = "10.0"
+        os.environ["TORCH_CUDA_ARCH_LIST"] = "9.0"
         from torch.utils.cpp_extension import load
         root = os.path.join(REF, "optimum/quanto/library/extensions/cuda")
         sources = ["unpack.cu", "awq/v2/gemm_cuda.cu", "awq/v2/gemv_cuda.cu", "marlin/fp8_marlin.cu",
@@ -50,13 +50,13 @@ def main():
                    "pybind_module.cpp"]
         build = os.path.join(root, "build")
         os.makedirs(build, exist_ok=True)
-        # the flags of optimum/quanto/library/extensions/cuda/__init__.py:47-55 on a B200 (capability 10.0 -> "1000")
+        # the flags of optimum/quanto/library/extensions/cuda/__init__.py:47-55 on an H100 (capability 9.0 -> "900")
         load(name="quanto_cuda", sources=[f"{root}/{s}" for s in sources], extra_cflags=["-g", "-O3"],
-             extra_cuda_cflags=["--expt-extended-lambda", "--use_fast_math", "-DQUANTO_CUDA_ARCH=1000"],
+             extra_cuda_cflags=["--expt-extended-lambda", "--use_fast_math", "-DQUANTO_CUDA_ARCH=900"],
              build_directory=build, verbose=True)
         with open(os.path.join(build, "pytorch_version.txt"), "w") as f:
             f.write(torch.__version__)
-        print("quanto_cuda built for sm_100")
+        print("quanto_cuda built for sm_90")
 
 
 if __name__ == "__main__":

@@ -303,7 +303,7 @@ def qbytes_mm_fp8_native(a_bits: np.ndarray, a_tag: str, w_bits: np.ndarray, w_t
     """Exact-math statement of the fp8 x fp8 tensor path: rnd_tag(fp32(sum a*w) * scales[n]).
 
     This is NOT the reference's rounding order (which rounds scales*W to the output dtype first,
-    qbytes_mm.py:31-33); it is the oracle for the native tcgen05 kind::f8f6f4 kernel, whose distance
+    qbytes_mm.py:31-33); it is the oracle for the fp8 x fp8 tensor-core kernel, whose distance
     to the reference is bounded separately in the tests.
     """
     a = fp8_bits_to_f32(a_bits, a_tag).astype(np.float64)

@@ -2,8 +2,8 @@
 
 The small-shape suites (test_gpu_cabi.py) never make a persistent CTA process more than one tile; these tests run the
 Llama-3-8B shapes (M = 4096, N = 14336 / 4096, K = 4096 / 14336), where every CTA loops over 2-7 tiles: accumulator
-hand-back, mbarrier phase wrap, the staging groups' tile stepping, both tile widths (224 / 256), both epilogues
-(per-lane stores / staged TMA stores) and the CTA-pair kernels are all executed and checked.
+mbarrier phase wrap, the staging groups' tile stepping and both tile heights (one or two consumer warpgroups) are all
+executed and checked.
 
 How a 4096 x 14336 x 4096 product is checked against the CPU oracle in seconds:
 * the operands: the kernel's dequantisation is bit-exact against the oracle on the WHOLE weight (the standalone
@@ -108,11 +108,8 @@ INT4_CASES = [
 # kernel variants: (label, override key, value) -- every one must give the same operands and pass the same bounds
 INT4_VARIANTS = [
     ("auto", None, None),
-    ("tile224", "OVR_INT4_TILE_N", 224),
-    ("tile256_tma_store", "OVR_EPILOGUE", 2),
-    ("tile256_lane_store", ("OVR_INT4_TILE_N", "OVR_EPILOGUE"), (256, 1)),
-    ("cta_pair", "OVR_INT4_ROUTE", 5),
-    ("cta_pair_tmem", "OVR_INT4_ROUTE", 6),
+    ("tile_m64", "OVR_TILE_M", 64),
+    ("tile_m128", "OVR_TILE_M", 128),
 ]
 
 
@@ -138,8 +135,8 @@ def test_int4_bench_shapes_all_kernel_variants(M, N, K, tag, zeropoint, bias):
         oracle.check(y, (label, M, N, K, tag))
         check_full_against_device_fp32(y, dev["x"], deq_gpu, dev["bias"], (label, M, N, K, tag))
         outs[label] = y
-    # same operands, same k order inside a tile: the single-CTA variants are bit-identical to each other
-    assert torch.equal(outs["tile256_tma_store"], outs["tile256_lane_store"])
+    # same operands, same k order inside a tile: both tile heights are bit-identical to each other
+    assert torch.equal(outs["tile_m64"], outs["tile_m128"])
     # through the QTensor / F.linear surface: the same launch
     import quanto_b200 as q
     rows_g = N * K // 128
@@ -152,8 +149,8 @@ def test_int4_bench_shapes_all_kernel_variants(M, N, K, tag, zeropoint, bias):
 
 @pytest.mark.parametrize("M", [33, 64, 100, 128])
 @pytest.mark.parametrize("tag", ["bf16", "f16"])
-def test_int4_tcgen05_decode_kernel_llama_shapes(M, tag):
-    """32 < M <= 128: the tcgen05 kernel with the weight operand in tensor memory, at N = 14336 and K = 14336."""
+def test_int4_mid_m_llama_shapes(M, tag):
+    """32 < M <= 128: the wgmma kernel (one or two consumer warpgroups), at N = 14336 and K = 14336."""
     n = native()
     lib = n.load()
     for (N, K) in ((14336, 4096), (4096, 14336)):
@@ -176,7 +173,7 @@ def test_int4_small_m_routes_agree(M):
     N, K, tag = 14336, 4096, "bf16"
     x_bits, deq_bits, bias_bits, dev, _ = int4_case(M, N, K, 128, tag, False, M == 16, seed=M)
     oracle = RowOracle(np.arange(M), x_bits, deq_bits, bias_bits, tag)
-    routes = (0, n.ROUTE_INT4_GEMV, n.ROUTE_INT4_TCDECODE, n.ROUTE_INT4_GENERAL) + ((n.ROUTE_INT4_RING2,) if M <= 16 else ())
+    routes = (0, n.ROUTE_INT4_GEMV, n.ROUTE_INT4_GENERAL) + ((n.ROUTE_INT4_RING2,) if M <= 16 else ())
     for route in routes:
         with n.test_override(n.OVR_INT4_ROUTE, route):
             y = cabi_qbits_mm(dev["x"], dev["packed"], dev["scale"], dev["shift"], dev["bias"], N, K, 128)
@@ -207,7 +204,7 @@ def _int_product_on_device(A, W):
 
 
 @pytest.mark.parametrize("N", [4096, 14336])
-@pytest.mark.parametrize("variant", ["auto", "tile224", "tile256", "single_cta"])
+@pytest.mark.parametrize("variant", ["auto", "tile128", "tile256", "tile_m64"])
 def test_int8_bench_shapes_bit_exact(N, variant):
     n = native()
     lib = n.load()
@@ -220,8 +217,8 @@ def test_int8_bench_shapes_bit_exact(N, variant):
     At, Wt = torch.from_numpy(A).cuda(), torch.from_numpy(W).cuda()
     st = bits_to_torch(O.from_f32(s, tag), tag)
     bt = None if bias is None else bits_to_torch(O.from_f32(bias, tag), tag)
-    key, val = {"auto": (None, 0), "tile224": (n.OVR_QBYTES_TILE_N, 224), "tile256": (n.OVR_QBYTES_TILE_N, 256),
-                "single_cta": (n.OVR_QBYTES_ROUTE, n.ROUTE_QBYTES_SINGLE)}[variant]
+    key, val = {"auto": (None, 0), "tile128": (n.OVR_QBYTES_TILE_N, 128), "tile256": (n.OVR_QBYTES_TILE_N, 256),
+                "tile_m64": (n.OVR_TILE_M, 64)}[variant]
     try:
         if key is not None:
             lib.qb200_test_override(key, val)
@@ -327,7 +324,7 @@ def test_second_device_in_one_process():
 def test_fused_gather_emulated_on_one_gpu(M, world):
     """The column-parallel kernels with the all-gather fused in (qb200_qbits_mm_gather), exercised on ONE device: the
     `world` "ranks" are `world` output buffers and flag arrays on the same GPU and the ranks' kernels run one after the
-    other.  Checks the peer stores (every rank's slab lands in every buffer at its column offset, TMA-store epilogue for
+    other.  Checks the peer stores (every rank's slab lands in every buffer at its column offset, wgmma epilogue for
     M > 8, ring-gemv reducer for M <= 8), bit-identity with the single-rank linear on the full weight, and the flag
     protocol (epochs published to every flag array; a kernel that waits for its input passes once all ranks published)."""
     import ctypes

@@ -387,7 +387,7 @@ def test_qbytes_mm_int8_exact(tag, M, N, K):
 @pytest.mark.parametrize("tag", ["bf16", "f16", "f32"])
 @pytest.mark.parametrize("M,N,K", [(512, 2048, 4096), (1024, 1024, 512), (384, 4096, 256)])
 def test_qbytes_mm_int8_fused_bias_large(tag, M, N, K):
-    """Bias fused into the epilogue of the large-tile (CTA-pair) kernels: acc*scale rounded, then + bias rounded, exactly
+    """Bias fused into the epilogue of the wgmma kernels: acc*scale rounded, then + bias rounded, exactly
     the two roundings of the reference's `qbytes_mm(...) + bias` (tensor/weights/qbytes.py:68-82)."""
     rng = np.random.default_rng(M * 3 + N + K)
     A = rng.integers(-127, 128, size=(M, K), dtype=np.int8)
@@ -410,7 +410,7 @@ def test_qbytes_mm_int8_fused_bias_large(tag, M, N, K):
 @pytest.mark.parametrize("wkind", ["int8", "e4m3fn", "e5m2"])
 @pytest.mark.parametrize("M,N,K", [(7, 300, 128), (128, 512, 1024), (300, 640, 2048), (1000, 1024, 512)])
 def test_qbytes_mm_weight_only_tensor_path(tag, wkind, M, N, K):
-    """fp16/bf16 activations x int8/fp8 weights on tcgen05: operands rnd(scale*W) are bit-identical to the reference's
+    """fp16/bf16 activations x int8/fp8 weights on wgmma: operands rnd(scale*W) are bit-identical to the reference's
     python path (library/qbytes_mm.py:25-33); only the fp32 summation order may differ."""
     rng = np.random.default_rng(M + N + K)
     a = O.round_to(rng.standard_normal((M, K), dtype=np.float32), tag)

@@ -189,8 +189,8 @@ def _rand8(kind, shape, g):
 @pytest.mark.parametrize("M,N,K", [(64, 256, 128), (300, 512, 1024), (257, 300, 256), (1000, 1024, 512), (8, 48, 64)])
 @pytest.mark.parametrize("with_bias", [False, True])
 def test_qbytes_linear_quantized_is_the_composition(dtype, kind, out_dt, M, N, K, with_bias):
-    """One launch == qbytes_mm (+ bias) followed by quantize_symmetric, bit for bit; both kernel families (CTA pair for
-    M > 128, single CTA below), ragged N (element-wise stores), every scale dtype."""
+    """One launch == qbytes_mm (+ bias) followed by quantize_symmetric, bit for bit; both tile heights (128 rows for
+    M > 64, 64 rows below), ragged N (element-wise stores), every scale dtype."""
     from quanto_b200 import _native as n
     g = torch.Generator().manual_seed(M * 7 + N + K)
     a = _rand8(kind, (M, K), g).cuda()
@@ -203,7 +203,7 @@ def test_qbytes_linear_quantized_is_the_composition(dtype, kind, out_dt, M, N, K
     got = torch.ops.quanto.qbytes_linear_quantized(a, w, scales, bias, out_scale, out_dt)
     assert got.dtype == out_dt and got.shape == (M, N)
     assert torch.equal(got.view(torch.uint8), ref.view(torch.uint8)), float((got.view(torch.uint8) != ref.view(torch.uint8)).float().mean())
-    # and it really was the fused kernel (status 0 from the C entry point, tcgen05 family)
+    # and it really was the fused kernel (status 0 from the C entry point, wgmma family)
     lib = n.load()
     out = torch.empty((M, N), dtype=out_dt, device="cuda")
     rc = lib.qb200_qbytes_mm_quantized(n.ptr(a), n.ptr(w), n.ptr(scales.reshape(-1).contiguous()), n.ptr(bias), n.ptr(out),

@@ -360,10 +360,10 @@ def test_release_library_ignores_debug_flags_and_env():
 def test_test_override_keys_are_validated():
     from quanto_b200 import _native as n
     lib = n.load()
-    assert lib.qb200_test_override(n.OVR_INT4_TILE_N, 224) == 0
-    assert lib.qb200_test_override(n.OVR_INT4_TILE_N, 0) == 0
+    assert lib.qb200_test_override(n.OVR_TILE_M, 64) == 0
+    assert lib.qb200_test_override(n.OVR_TILE_M, 0) == 0
     assert lib.qb200_test_override(99, 1) == 1  # QB200_ERR_ARG
-    with n.test_override(n.OVR_EPILOGUE, 2):
+    with n.test_override(n.OVR_QBYTES_TILE_N, 256):
         pass
 
 
@@ -383,7 +383,7 @@ def test_ring_gemv_cut_of_k_does_not_depend_on_n():
                 for m in range(1, 17):
                     cuts = set()
                     for N in (16, 256, 512, 1024, 1792, 2048, 3584, 4096, 7168, 14336, 28672, 128256):
-                        for grid in (148, 132):
+                        for grid in (132, 114):
                             if lib.qb200_qbits_ring_plan(m, N, k, group, zp, grid, out):
                                 cuts.add((out[0], out[1], out[3]))
                                 assert out[4] <= 227 * 1024 and out[2] >= 2
@@ -391,8 +391,8 @@ def test_ring_gemv_cut_of_k_does_not_depend_on_n():
                     seen += len(cuts)
     assert seen > 200  # the kernel takes most of these problems
     # the shapes of the Llama-3-8B decode step at batch 1 and 8 run on it, the K = 14336 projection at batch 8 in passes
-    assert lib.qb200_qbits_ring_plan(1, 14336, 4096, 128, 0, 148, out) and (out[0], out[1]) == (4, 1)
-    assert lib.qb200_qbits_ring_plan(8, 4096, 14336, 128, 0, 148, out) and out[1] > 1
+    assert lib.qb200_qbits_ring_plan(1, 14336, 4096, 128, 0, 132, out) and (out[0], out[1]) == (4, 1)
+    assert lib.qb200_qbits_ring_plan(8, 4096, 14336, 128, 0, 132, out) and out[1] > 1
 
 
 @pytest.mark.parametrize("world", [2, 4, 8])

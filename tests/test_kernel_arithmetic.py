@@ -3,7 +3,7 @@ csrc/freeze.cu), checked against the oracle.  The kernels must be bit-exact with
 do not execute it literally: they multiply by a reciprocal instead of dividing, round through a magic-number addition
 instead of cvt instructions, and (bf16) stay in packed 16-bit arithmetic.  Each identity used is pinned here, without a
 GPU; an earlier draft of the zero-point path (zero-point folded into the rounding constant) failed exactly this check
-before it ever ran on a B200.
+before it ever ran on a GPU.
 """
 import numpy as np
 

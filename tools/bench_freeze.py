@@ -47,7 +47,7 @@ def main():
     ws = [(torch.randn(N, K, device=dev) * 0.02).to(torch.bfloat16) for _ in range(nrot)]
     rows = N * K // G
 
-    if "--ncu" in sys.argv:  # a few launches of the kernels profiled under ncu (profiles/r1_freeze_ncu_summary.json)
+    if "--ncu" in sys.argv:  # a few launches of the kernels, for a profiler
         xs = torch.randn(4096, 4096, device=dev, dtype=torch.bfloat16)
         sc = torch.tensor(0.03, device=dev, dtype=torch.bfloat16)
         for i in range(3):

@@ -1,6 +1,6 @@
 """Multi-rank check (torchrun, NCCL): column-parallel QLinear == single-GPU QLinear, BIT FOR BIT, for
 * sharded canonical int4 weights + NCCL all-gather (`gather_columns`),
-* the all-gather and rank synchronisation fused into the kernel (`FusedGather`: ring gemv M <= 8, stream-K tcgen05 kernel
+* the all-gather and rank synchronisation fused into the kernel (`FusedGather`: ring gemv M <= 8, wgmma kernel
   8 < M <= 128 -- tolerance there, its split of K depends on the shard shape --, persistent GEMM M > 128),
 * a CHAIN of fused linears that synchronise only through the in-kernel flags (wait_input / no wait_output), eager and
   replayed from a CUDA graph.
@@ -84,7 +84,7 @@ for M in (1, 8, 32, 512):
 
     # bit-identity needs kernels whose k-order does not depend on the shard shape: the ring gemv (whole-K ownership,
     # several passes over K when the activations do not fit shared memory; M <= 8) and the large-M GEMMs; the stream-K
-    # tcgen05 decode kernel in between is checked against a tolerance
+    # wgmma kernel in between is checked against a tolerance
     exact = M <= 8 or M > 128
     same_fn = torch.equal if exact else close
     good = True

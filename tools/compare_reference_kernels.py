@@ -1,7 +1,7 @@
 """Same-box comparison against the kernels the REFERENCE ITSELF dispatches to on this GPU (SURVEY 2.2 / BASELINE.md 5).
 
 Runs the unmodified reference from oracle/_ref (python oracle/build_ref.py; its `quanto_cuda` extension -- AWQ v2, Marlin
-FP8 -- pre-built for sm_100) in one process and this library in another, on the same Llama-3-8B shapes, CUDA-graph replay
+FP8 -- pre-built for sm_90) in one process and this library in another, on the same Llama-3-8B shapes, CUDA-graph replay
 over rotated weight copies (HBM-cold), CUDA events.  Reference routes (optimum/quanto/tensor/weights/qbits.py:97-138,
 qbytes.py:122-143, library/qbytes_mm.py:73-88):
   fp16 x qint4 g128       -> AWQWeightQBitsTensor    -> quanto::gemm_f16i4_awq   (gemv rows < 8, else gemm; mma.sync)
@@ -45,7 +45,7 @@ def graph_time_us(torch, fns, reps=10):
 
 def arm_ref(part):
     sys.path.insert(0, REF)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0")
     import torch
     import optimum.quanto as oq
     from optimum.quanto import AbsmaxOptimizer, MaxOptimizer, qfloat8_e4m3fn, qint4, qint8

@@ -1,4 +1,4 @@
-"""pytest plugin (`-p quanto_b200_bind`): bind the sm_100a kernels into the imported reference before its tests run."""
+"""pytest plugin (`-p quanto_b200_bind`): bind the sm_90a kernels into the imported reference before its tests run."""
 import optimum.quanto  # noqa: F401
 
 from quanto_b200.integration import bind_reference

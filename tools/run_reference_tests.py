@@ -1,4 +1,4 @@
-"""Run the reference's OWN hot-path tests against the sm_100a kernels (SURVEY 4: "still pass the reference's tests").
+"""Run the reference's OWN hot-path tests against the sm_90a kernels (SURVEY 4: "still pass the reference's tests").
 
 Needs oracle/_ref (python oracle/build_ref.py in the authoring container: the unmodified reference + its tests, git-ignored,
 travels to the GPU box).  The kernels are bound into the real `optimum.quanto` classes by quanto_b200.integration.
@@ -24,7 +24,7 @@ def main():
     env = dict(os.environ)
     env["PYTHONPATH"] = os.pathsep.join([REF, os.path.join(ROOT, "optimum-quanto_b200"), os.path.join(ROOT, "tools"),
                                          env.get("PYTHONPATH", "")])
-    env["TORCH_CUDA_ARCH_LIST"] = "10.0"
+    env["TORCH_CUDA_ARCH_LIST"] = "9.0"
     sel = ["library/test_unpack.py", "library/test_quantize.py", "library/test_mm.py::test_qbytes_mm",
            "tensor/test_packed_tensor.py", "tensor/ops/test_linear_dispatch.py",
            "tensor/weights/test_weight_qbits_tensor_dispatch.py", "tensor/weights/test_weight_qbits_tensor_quantize.py",

@@ -14,8 +14,7 @@ for N in (14336, 7168, 3584, 1792):
     packed = torch.randint(0, 256, (N // 2, K), dtype=torch.uint8, device=dev)
     scale = (torch.rand(N * K // G, device=dev) * 0.01 + 0.002).to(torch.bfloat16)
     shift = (scale.float() * 8).to(torch.bfloat16)
-    for name, fl in (("single-CTA tiles", 0), ("CTA-pair tiles", 128)):
-        lib.qb200_debug_set_flags(fl)
-        t = timeit(lambda: cabi_qbits_mm(x, packed, scale, shift, None, N, K, G, use_workspace=False), iters=20)
+    for name, rows in (("64-row tiles", 64), ("128-row tiles", 128)):
+        with native().test_override(native().OVR_TILE_M, rows):
+            t = timeit(lambda: cabi_qbits_mm(x, packed, scale, shift, None, N, K, G, use_workspace=False), iters=20)
         print(f"N={N:6d} {name:18s} {t*1e6:8.1f} us  {2*M*N*K/t/1e12:7.1f} TF/s", flush=True)
-lib.qb200_debug_set_flags(0)
