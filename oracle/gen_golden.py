@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 import optimum.quanto  # noqa: F401  (registers torch.ops.quanto.*)
-from optimum.quanto import MaxOptimizer, qint2, qint4, qint8, qfloat8_e4m3fn, qfloat8_e5m2
+from optimum.quanto import MaxOptimizer, qint2, qint4, qint8, qfloat8_e4m3fn, qfloat8_e4m3fnuz, qfloat8_e5m2
 from optimum.quanto.tensor.packed import pack_weights
 from optimum.quanto.tensor.weights import quantize_weight
 
@@ -26,7 +26,7 @@ OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "g
 os.makedirs(OUT, exist_ok=True)
 
 TAG = {torch.float32: "f32", torch.float16: "f16", torch.bfloat16: "bf16"}
-F8TAG = {torch.float8_e4m3fn: "e4m3fn", torch.float8_e5m2: "e5m2"}
+F8TAG = {torch.float8_e4m3fn: "e4m3fn", torch.float8_e5m2: "e5m2", torch.float8_e4m3fnuz: "e4m3fnuz"}
 
 
 def bits(t: torch.Tensor) -> np.ndarray:
@@ -331,10 +331,120 @@ def gen_affine_zp(g):
     np.savez_compressed(os.path.join(OUT, "affine_zp.npz"), **cases)
 
 
+def gen_fnuz(g):
+    """float8_e4m3fnuz (bias 8, max 240, 0x80 = NaN, no negative zero) through the reference's own entry points:
+    quantize_symmetric to it (all-zero rows, quotients past +-240, tiny negatives), qbytes_mm with e4m3fnuz weights
+    (the reference's tests/library/test_mm.py "w-float8-uz" cases) and two frozen QLinear layers.  A separate file with
+    its own seed: the fixtures committed earlier stay byte-identical."""
+    from optimum.quanto.nn import QLinear
+
+    fnuz = torch.float8_e4m3fnuz
+    cases = {}
+    idx = 0
+    for in_dtype in (torch.float32, torch.float16, torch.bfloat16):
+        for axis, shape in ((None, (37, 64)), (0, (48, 96)), (-1, (48, 96))):
+            base = (torch.rand(shape, generator=g) * 2 - 1) * 3
+            base[:, :4] *= 1e-5  # |quotient| below half the smallest subnormal (2^-11): +-0 -> 0x00, never 0x80
+            if axis is None:
+                base = base.to(in_dtype)
+                scale = (base.abs().max().float() / 300).to(in_dtype)  # quotients up to +-300: clamped to +-240
+            elif axis == 0:
+                base[5] = 0  # all-zero row: scale 0, quotient 0/0 -> NaN -> 0x80
+                base = base.to(in_dtype)
+                scale = (base.abs().amax(dim=1, keepdim=True).float() / 240).to(in_dtype)
+            else:
+                base = base.to(in_dtype)
+                scale = (base.abs().amax(dim=0, keepdim=True).float() / 260).to(in_dtype)
+            out = torch.ops.quanto.quantize_symmetric(base, dtype=fnuz, axis=axis, scale=scale)
+            p = f"q{idx}_"
+            cases[p + "in_tag"] = np.array(TAG[in_dtype])
+            cases[p + "axis"] = np.int64(-2 if axis is None else axis)
+            cases[p + "base"] = bits(base)
+            cases[p + "scale"] = bits(scale)
+            cases[p + "out"] = bits(out)
+            idx += 1
+    cases["n_quantize"] = np.int64(idx)
+    idx = 0
+    # (activation kind, out dtype, M, K, N): "same" = activations in the output dtype
+    for akind, odt, M, K, N in [
+        ("same", torch.float16, 32, 32, 48),
+        ("same", torch.bfloat16, 32, 64, 50),
+        ("same", torch.float16, 10, 80, 64),
+        ("same", torch.bfloat16, 10, 80, 48),
+        ("f32", torch.bfloat16, 16, 64, 48),
+        ("int8", torch.float16, 32, 50, 64),
+        ("int8", torch.bfloat16, 10, 64, 50),
+        ("e4m3fnuz", torch.float16, 16, 64, 48),
+    ]:
+        if akind == "int8":
+            A = torch.randint(-127, 127, (M, K), dtype=torch.int8, generator=g)
+        elif akind == "e4m3fnuz":
+            A = torch.randn(M, K, generator=g).to(fnuz)
+        else:
+            A = (torch.rand(M, K, generator=g) * 2 - 1).to(odt if akind == "same" else torch.float32)
+        W = (torch.randn(N, K, generator=g) * 20).clamp(-240, 240).to(fnuz)
+        scales = (torch.rand(N, 1, generator=g) / 1e3 + 1e-5).to(odt)
+        y = torch.ops.quanto.qbytes_mm(A, W, scales)
+        p = f"m{idx}_"
+        cases[p + "akind"] = np.array(akind)
+        cases[p + "tag"] = np.array(TAG[odt])
+        cases[p + "A"] = bits(A)
+        cases[p + "W"] = bits(W)
+        cases[p + "scales"] = bits(scales)
+        cases[p + "y"] = bits(y)
+        idx += 1
+    cases["n_mm"] = np.int64(idx)
+    idx = 0
+    for dtype, wq, aq, K, N, M in [
+        (torch.float16, qfloat8_e4m3fnuz, None, 128, 64, 8),
+        (torch.bfloat16, qint8, qfloat8_e4m3fnuz, 128, 64, 32),
+    ]:
+        lin = torch.nn.Linear(K, N, bias=True).to(dtype)
+        with torch.no_grad():
+            lin.weight.copy_((torch.randn(N, K, generator=g) * 0.05).to(dtype))
+            lin.bias.copy_((torch.randn(N, generator=g) * 0.1).to(dtype))
+        q = QLinear.from_module(lin, weights=wq, activations=aq)
+        x = torch.randn(M, K, generator=g).to(dtype)
+        if aq is not None:
+            q.input_scale = (x.abs().max().float() / 240.0).to(dtype)
+            with torch.no_grad():
+                y_float = lin(x)
+            q.output_scale = (y_float.abs().max().float() / 240.0).to(dtype)
+        qw = q.qweight  # canonical tensors, as in gen_qlinear
+        if type(qw).__name__ != "WeightQBytesTensor":
+            qw = qw.weight_qbytes_tensor()
+        q.weight = torch.nn.Parameter(qw)
+        with torch.no_grad():
+            y = q(x)
+        p = f"l{idx}_"
+        cases[p + "tag"] = np.array(TAG[dtype])
+        cases[p + "wq"] = np.array(wq.name)
+        cases[p + "aq"] = np.array("none" if aq is None else aq.name)
+        cases[p + "x"] = bits(x)
+        cases[p + "bias"] = bits(lin.bias)
+        cases[p + "input_scale"] = bits(q.input_scale.reshape(1))
+        cases[p + "output_scale"] = bits(q.output_scale.reshape(1))
+        for k, v in q.state_dict().items():
+            if k.startswith("weight"):
+                cases[p + "sd_" + k] = bits(v)
+        cases[p + "shape"] = np.array([N, K, M, 0], dtype=np.int64)
+        if aq is None:
+            cases[p + "y"] = bits(y)
+        else:
+            cases[p + "y_data"] = bits(y._data)
+            cases[p + "y_scale"] = bits(y._scale.reshape(1))
+        idx += 1
+    cases["n_qlinear"] = np.int64(idx)
+    np.savez_compressed(os.path.join(OUT, "fnuz.npz"), **cases)
+
+
 def main():
     torch.set_num_threads(1)  # deterministic accumulation order for the stored float results
     if "--affine-zp-only" in sys.argv:  # added in round 2 (a bug found by the reference's own tests): new file only
         gen_affine_zp(torch.Generator().manual_seed(20260924))
+        return 0
+    if "--fnuz-only" in sys.argv:  # added with the float8_e4m3fnuz coverage: new file only
+        gen_fnuz(torch.Generator().manual_seed(20261017))
         return 0
     if "--freeze-only" in sys.argv:  # added after the first fixtures were committed: keeps those byte-identical
         gen_freeze(torch.Generator().manual_seed(20260923))
@@ -347,6 +457,7 @@ def main():
     gen_qlinear(g)
     gen_freeze(torch.Generator().manual_seed(20260923))
     gen_affine_zp(torch.Generator().manual_seed(20260924))
+    gen_fnuz(torch.Generator().manual_seed(20261017))
     tot = sum(os.path.getsize(os.path.join(OUT, f)) for f in os.listdir(OUT))
     print("wrote fixtures to", os.path.normpath(OUT), f"({tot/1024:.0f} KiB)")
 

@@ -24,7 +24,7 @@ import numpy as np
 # dtype helpers: every low precision format <-> float32, RNE
 # --------------------------------------------------------------------------
 FLOAT_TAGS = ("f32", "f16", "bf16")
-FP8_TAGS = ("e4m3fn", "e5m2")
+FP8_TAGS = ("e4m3fn", "e5m2", "e4m3fnuz")
 
 
 def bf16_bits_to_f32(bits: np.ndarray) -> np.ndarray:
@@ -80,11 +80,17 @@ def round_to(x: np.ndarray, tag: str) -> np.ndarray:
 
 
 def _fp8_table(tag: str) -> np.ndarray:
-    """Decode table for the 128 non-negative codes of an fp8 format (NaN/inf -> nan)."""
+    """Decode table for the 128 non-negative codes of an fp8 format (NaN/inf -> nan).
+
+    e4m3fnuz (torch.float8_e4m3fnuz): bias 8, no infinities, all 128 codes finite; its only NaN is 0x80, the code
+    that would be negative zero (see fp8_bits_to_f32).
+    """
     if tag == "e4m3fn":
         ebits, mbits, bias = 4, 3, 7
     elif tag == "e5m2":
         ebits, mbits, bias = 5, 2, 15
+    elif tag == "e4m3fnuz":
+        ebits, mbits, bias = 4, 3, 8
     else:
         raise ValueError(tag)
     out = np.empty(128, dtype=np.float64)
@@ -104,17 +110,24 @@ def _fp8_table(tag: str) -> np.ndarray:
 
 
 _FP8_TABLES = {t: _fp8_table(t) for t in FP8_TAGS}
-FP8_MAX = {"e4m3fn": 448.0, "e5m2": 57344.0}
+FP8_MAX = {"e4m3fn": 448.0, "e5m2": 57344.0, "e4m3fnuz": 240.0}
 
 
 def fp8_bits_to_f32(bits: np.ndarray, tag: str) -> np.ndarray:
     b = np.asarray(bits, dtype=np.uint8)
     mag = _FP8_TABLES[tag][b & 0x7F]
-    return np.where(b & 0x80, -mag, mag).astype(np.float32)
+    out = np.where(b & 0x80, -mag, mag)
+    if tag == "e4m3fnuz":
+        out = np.where(b == 0x80, np.nan, out)
+    return out.astype(np.float32)
 
 
 def f32_to_fp8_bits(x: np.ndarray, tag: str) -> np.ndarray:
-    """RNE float32 -> fp8 for finite inputs with |x| <= finfo.max (callers clamp first)."""
+    """RNE float32 -> fp8 for finite inputs with |x| <= finfo.max (callers clamp first).
+
+    e4m3fnuz has no negative zero: a zero of either sign, and a negative value that rounds to zero, encode as 0x00;
+    NaN encodes as 0x80 (torch's cast).
+    """
     x = np.asarray(x, dtype=np.float32)
     table = _FP8_TABLES[tag]
     ncodes = int(np.sum(np.isfinite(table)))  # finite magnitudes are codes [0, ncodes)
@@ -129,6 +142,9 @@ def f32_to_fp8_bits(x: np.ndarray, tag: str) -> np.ndarray:
     code = np.where(pick_hi, hi, lo).astype(np.uint8)
     code = np.where(a == finite[hi], hi, code).astype(np.uint8)
     sign = (np.signbit(x)).astype(np.uint8) << 7
+    if tag == "e4m3fnuz":
+        sign = np.where(code == 0, np.uint8(0), sign)
+        return np.where(np.isnan(x), np.uint8(0x80), code | sign).astype(np.uint8)
     code = np.where(np.isnan(x), np.uint8(0x7F), code)  # torch keeps NaN (0/0 of an all-zero row) as the NaN code
     return (code | sign).astype(np.uint8)
 
@@ -206,7 +222,8 @@ def quantize_symmetric(base_f32: np.ndarray, in_tag: str, out_tag: str, scale_f3
     `base_f32`/`scale_f32` hold values already representable in `in_tag`; scale is
     broadcastable to base (scalar, [N,1] for axis 0, [1,N] for axis -1).
     t = round_to_in_dtype(base / scale)   (the division result is rounded to the INPUT dtype)
-    int8: rint (half-to-even), clamp [-128,127]; fp8: clamp to +-finfo.max then RNE cast.
+    int8: rint (half-to-even), clamp [-128,127]; fp8: clamp to +-finfo.max then RNE cast (the clamp matters for
+    e4m3fnuz: torch's cast maps values past 248 to NaN instead of saturating).
     Returns int8 array or fp8 bit patterns (uint8).
     """
     with np.errstate(divide="ignore", invalid="ignore", over="ignore"):

@@ -13,7 +13,8 @@ for p in (ROOT, os.path.join(ROOT, "optimum-quanto_b200")):
 from oracle import quanto_oracle as O  # noqa: E402
 
 TORCH_DT = {"f32": torch.float32, "f16": torch.float16, "bf16": torch.bfloat16,
-            "e4m3fn": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2, "int8": torch.int8}
+            "e4m3fn": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2, "e4m3fnuz": torch.float8_e4m3fnuz,
+            "int8": torch.int8}
 TAG_OF = {v: k for k, v in TORCH_DT.items()}
 
 
@@ -24,7 +25,7 @@ def bits_to_torch(arr: np.ndarray, tag: str, device="cuda") -> torch.Tensor:
     if tag in ("f16", "bf16"):
         t = torch.from_numpy(np.ascontiguousarray(arr).view(np.int16)).to(device)
         return t.view(TORCH_DT[tag])
-    if tag in ("e4m3fn", "e5m2"):
+    if tag in O.FP8_TAGS:
         t = torch.from_numpy(np.ascontiguousarray(arr).view(np.uint8)).to(device)
         return t.view(TORCH_DT[tag])
     if tag == "int8":
@@ -40,7 +41,7 @@ def torch_to_bits(t: torch.Tensor) -> np.ndarray:
         return t.numpy()
     if t.dtype in (torch.float16, torch.bfloat16):
         return t.view(torch.int16).numpy().view(np.uint16)
-    if t.dtype in (torch.float8_e4m3fn, torch.float8_e5m2):
+    if t.dtype in (torch.float8_e4m3fn, torch.float8_e5m2, torch.float8_e4m3fnuz):
         return t.view(torch.uint8).numpy()
     return t.numpy()
 
@@ -135,3 +136,54 @@ def make_qbits_weights(N, K, group, tag, seed=0, zeropoint=False):
     else:
         shift = O.from_f32(O.to_f32(scale, tag) * (7.0 + 2 * rng.random(rows, dtype=np.float32)), tag)
     return q, packed, scale, shift
+
+
+def band_rows(M, seed, per_band=2):
+    """`per_band` distinct rows of every 32-row band of [0, M): every tile / epilogue warp of any tiling is sampled."""
+    rng = np.random.default_rng(seed)
+    rows = []
+    for b0 in range(0, M, 32):
+        hi = min(32, M - b0)
+        rows.extend((b0 + rng.choice(hi, size=min(per_band, hi), replace=False)).tolist())
+    return np.array(sorted(rows), dtype=np.int64)
+
+
+def check_full_against_device_fp32(y_gpu, x_t, w_t, bias_t, label):
+    """All output elements against the fp32 product of the same operands (cuBLAS fp32, TF32 off), rounded the way the
+    reference rounds.  Catches a misplaced / stale / skipped tile anywhere in the output."""
+    prev = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        ref = torch.matmul(x_t.float(), w_t.float().t()).to(y_gpu.dtype)
+        if bias_t is not None:
+            ref = (ref + bias_t).to(y_gpu.dtype)
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev
+    d = (y_gpu.float() - ref.float())
+    rel = float(d.norm() / ref.float().norm())
+    assert rel < 1e-3, (label, rel)
+    # per element: two results of the same exact sum rounded to the output dtype differ by at most one output ulp plus
+    # the accumulation-order slack; 2^-6 relative + a small absolute floor is ~4 bf16 ulps
+    tol = ref.float().abs() * 2.0 ** -6 + 2.0 ** -6 * ref.float().abs().mean()
+    bad = int((d.abs() > tol).sum())
+    assert bad == 0, (label, bad, float((d.abs() / tol).max()))
+    return float((y_gpu == ref).float().mean())
+
+
+def check_linear(y_gpu, x_bits, deq_bits, bias_bits, tag, label):
+    """A linear of dequantised operands against the float64 oracle: per-element bound and norm error vs the
+    reference-rounded result.  Returns the fraction of bit-identical outputs."""
+    x = O.to_f32(x_bits, tag)
+    w = O.to_f32(deq_bits, tag)
+    bias = None if bias_bits is None else O.to_f32(bias_bits, tag)
+    y64, y_ref, tol = O.linear_from_dequantized(x, w, bias, tag)
+    y = torch_to_f32(y_gpu).astype(np.float64)
+    # rounding allowance (half an output ulp per rounding step) + fp32 accumulation-order slack
+    bound = 1.02 * tol + O.accumulate_allowance(x, w)
+    err = np.abs(y - y64)
+    assert np.all(err <= bound), (label, float(np.max(err / bound)), np.unravel_index(np.argmax(err / bound), err.shape))
+    # versus the reference-rounded result: same numbers up to accumulation order => norm error << 1e-3
+    yr = O.to_f32(y_ref, tag).astype(np.float64)
+    rel = np.linalg.norm(y - yr) / max(np.linalg.norm(yr), 1e-30)
+    assert rel < 1e-3, (label, rel)
+    return float(np.mean(torch_to_bits(y_gpu) == y_ref))

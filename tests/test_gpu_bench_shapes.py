@@ -20,20 +20,10 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import (O, bits_to_torch, cabi_dequantize_qbits, cabi_qbits_mm, cabi_qbytes_mm, make_qbits_weights, native,
-                     torch_to_bits, torch_to_f32)
+from helpers import (O, band_rows, bits_to_torch, cabi_dequantize_qbits, cabi_qbits_mm, cabi_qbytes_mm,
+                     check_full_against_device_fp32, make_qbits_weights, native, torch_to_bits, torch_to_f32)
 
 pytestmark = pytest.mark.gpu
-
-
-def band_rows(M, seed, per_band=2):
-    """`per_band` distinct rows of every 32-row band of [0, M): every tile / epilogue warp of any tiling is sampled."""
-    rng = np.random.default_rng(seed)
-    rows = []
-    for b0 in range(0, M, 32):
-        hi = min(32, M - b0)
-        rows.extend((b0 + rng.choice(hi, size=min(per_band, hi), replace=False)).tolist())
-    return np.array(sorted(rows), dtype=np.int64)
 
 
 class RowOracle:
@@ -59,28 +49,6 @@ class RowOracle:
 
 def check_rows_linear(y_gpu, rows, x_bits, deq_bits, bias_bits, tag, label):
     RowOracle(rows, x_bits, deq_bits, bias_bits, tag).check(y_gpu, label)
-
-
-def check_full_against_device_fp32(y_gpu, x_t, w_t, bias_t, label):
-    """All output elements against the fp32 product of the same operands (cuBLAS fp32, TF32 off), rounded the way the
-    reference rounds.  Catches a misplaced / stale / skipped tile anywhere in the output."""
-    prev = torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cuda.matmul.allow_tf32 = False
-    try:
-        ref = torch.matmul(x_t.float(), w_t.float().t()).to(y_gpu.dtype)
-        if bias_t is not None:
-            ref = (ref + bias_t).to(y_gpu.dtype)
-    finally:
-        torch.backends.cuda.matmul.allow_tf32 = prev
-    d = (y_gpu.float() - ref.float())
-    rel = float(d.norm() / ref.float().norm())
-    assert rel < 1e-3, (label, rel)
-    # per element: two results of the same exact sum rounded to the output dtype differ by at most one output ulp plus
-    # the accumulation-order slack; 2^-6 relative + a small absolute floor is ~4 bf16 ulps
-    tol = ref.float().abs() * 2.0 ** -6 + 2.0 ** -6 * ref.float().abs().mean()
-    bad = int((d.abs() > tol).sum())
-    assert bad == 0, (label, bad, float((d.abs() / tol).max()))
-    return float((y_gpu == ref).float().mean())
 
 
 def int4_case(M, N, K, G, tag, zeropoint, bias, seed):

@@ -7,6 +7,7 @@ import torch
 
 from helpers import (O, bits_to_torch, cabi_dequantize_qbits, cabi_qbits_mm, cabi_qbytes_mm, cabi_quantize_symmetric,
                      cabi_unpack, make_qbits_weights, torch_to_bits, torch_to_f32)
+from helpers import check_linear as _check_linear
 
 pytestmark = pytest.mark.gpu
 
@@ -106,23 +107,6 @@ def test_dequantize_qbits_golden(golden_dir):
         shift = torch.from_numpy(z[p + "shift"]).cuda().reshape(-1) if zp else bits_to_torch(z[p + "shift"], tag).reshape(-1)
         deq = cabi_dequantize_qbits(packed, scale, shift, N, K, G, int(z[p + "bits"]))
         assert np.array_equal(torch_to_bits(deq), z[p + "deq"]), (i, tag)
-
-
-def _check_linear(y_gpu, x_bits, deq_bits, bias_bits, tag, label):
-    x = O.to_f32(x_bits, tag)
-    w = O.to_f32(deq_bits, tag)
-    bias = None if bias_bits is None else O.to_f32(bias_bits, tag)
-    y64, y_ref, tol = O.linear_from_dequantized(x, w, bias, tag)
-    y = torch_to_f32(y_gpu).astype(np.float64)
-    # rounding allowance (half an output ulp per rounding step) + fp32 accumulation-order slack
-    bound = 1.02 * tol + O.accumulate_allowance(x, w)
-    err = np.abs(y - y64)
-    assert np.all(err <= bound), (label, float(np.max(err / bound)), np.unravel_index(np.argmax(err / bound), err.shape))
-    # versus the reference-rounded result: same numbers up to accumulation order => norm error << 1e-3
-    yr = O.to_f32(y_ref, tag).astype(np.float64)
-    rel = np.linalg.norm(y - yr) / max(np.linalg.norm(yr), 1e-30)
-    assert rel < 1e-3, (label, rel)
-    return float(np.mean(torch_to_bits(y_gpu) == y_ref))
 
 
 def test_qbits_mm_golden(golden_dir):

@@ -145,3 +145,79 @@ def test_int8_magic_rounding_path_equals_the_oracle():
             c = np.minimum(np.maximum(c, np.float32(-128)), np.float32(127))
             q = ((c + np.float32(12582912.0)).astype(np.float32).view(np.int32) & 0xFF).astype(np.uint8).view(np.int8)
         assert np.array_equal(q, ref)
+
+
+# ------------------------------------------------------------------------------------------- float8_e4m3fnuz
+def _emulate_fnuz_encode(t):
+    """quantize_one<DT_E4M3FNUZ> (csrc/quantize_math.cuh), statement by statement, on float32 quotients."""
+    t = np.asarray(t, np.float32)
+    with np.errstate(invalid="ignore"):
+        c = np.minimum(np.maximum(np.where(np.isnan(t), np.float32(0), t), np.float32(-240)), np.float32(240))
+    a = np.abs(c).astype(np.float32)
+    # subnormal branch: rint_bits(a * 1024) through the 1.5 * 2^23 addition
+    sub = ((a * np.float32(1024) + np.float32(12582912.0)).astype(np.float32).view(np.int32) - 0x4B400000).astype(np.uint32)
+    u = a.view(np.uint32).astype(np.uint32)
+    u = (u + np.uint32(0x7FFFF) + ((u >> 20) & 1)).astype(np.uint32)
+    nrm = (((((u >> 23) & 0xFF) - 119) << 3) | ((u >> 20) & 7)).astype(np.uint32)
+    b = np.where(a < np.float32(0.0078125), sub, nrm)
+    out = np.where(b == 0, 0, b | np.where(c < 0, 0x80, 0)).astype(np.uint8)
+    return np.where(np.isnan(t), np.uint8(0x80), out)
+
+
+def test_fnuz_kernel_encoder_equals_the_oracle():
+    """The hand-rolled RNE of the e4m3fnuz encoder == the oracle (pinned against torch's cast) for every finite bf16 and
+    fp16 value, every tie / subnormal boundary in fp32, values past +-240, +-inf, NaN and +-0."""
+    vals = [O.to_f32(np.arange(65536, dtype=np.uint16), tag) for tag in ("bf16", "f16")]
+    mags = np.sort(O.fp8_bits_to_f32(np.arange(128, dtype=np.uint8), "e4m3fnuz").astype(np.float64))
+    pts = np.concatenate([mags, (mags[:-1] + mags[1:]) / 2]).astype(np.float32)
+    pts = np.concatenate([pts, np.nextafter(pts, np.float32(np.inf)), np.nextafter(pts, np.float32(-np.inf)),
+                          np.float32([247.9, 248.0, 300.0, 3e38, np.inf, 2.0 ** -11, 1e-30, 0.0])])
+    vals.append(np.concatenate([pts, -pts]))
+    rng = np.random.default_rng(8)
+    vals.append((rng.standard_normal(300000) * 10.0 ** rng.uniform(-5, 3, 300000)).astype(np.float32))
+    for v in vals:
+        v = v[~np.isnan(v)]
+        ref = O.quantize_symmetric(v, "f32", "e4m3fnuz", np.float32(1.0))
+        assert np.array_equal(_emulate_fnuz_encode(v), ref), int(np.sum(_emulate_fnuz_encode(v) != ref))
+    assert _emulate_fnuz_encode(np.float32([np.nan, -0.0, -1e-6])).tolist() == [0x80, 0x00, 0x00]
+
+
+def _emulate_fnuz_stage(codes, s_bits, tag):
+    """cvt_bytes4<WT, 3> (csrc/gemm_tc.cuh): byte -> fp16 field pattern (bits << 7, sign to bit 15, the __vcmpeq2 patch
+    turning 0x80 into a NaN), x 128 in fp16, then rnd_WT(scale * w) -- fp16 directly, bf16 via half -> float -> bf16."""
+    t = np.asarray(codes, np.uint16)
+    h = ((t & 0x7F) << 7) | ((t & 0x80) << 8)
+    h = h | np.where(t == 0x80, 0x7FFF, 0).astype(np.uint16)
+    w16 = (h.astype(np.uint16).view(np.float16) * np.float16(128)).astype(np.float16)
+    if tag == "f16":
+        s = s_bits.astype(np.uint16).view(np.float16)
+        return (w16 * s).astype(np.float16).view(np.uint16)
+    w = O.round_to(w16.astype(np.float32), "bf16")
+    return O.from_f32((w * O.to_f32(s_bits, "bf16")).astype(np.float32), "bf16")
+
+
+def _emulate_fnuz_to_float(codes):
+    """e4m3fnuz_to_float (csrc/common.cuh), the decode of the CUDA-core qbytes_mm kernel."""
+    t = np.asarray(codes, np.uint16)
+    h = (((t & 0x7F) << 7) | ((t & 0x80) << 8)).astype(np.uint16)
+    v = h.view(np.float16).astype(np.float32) * np.float32(128)
+    return np.where(t == 0x80, np.float32(np.nan), v)
+
+
+def test_fnuz_staging_decoder_equals_the_oracle():
+    """Every one of the 256 codes times 2000 scales of each 16-bit type: the staged operand is the reference's
+    rnd(scale * W.to(dtype)) bit for bit (NaN for 0x80), and the CUDA-core decode is the oracle's table."""
+    codes = np.arange(256, dtype=np.uint8)
+    w = O.fp8_bits_to_f32(codes, "e4m3fnuz")
+    got = _emulate_fnuz_to_float(codes)
+    assert np.array_equal(np.isnan(got), np.isnan(w)) and np.array_equal(got[~np.isnan(w)], w[~np.isnan(w)])
+    rng = np.random.default_rng(9)
+    for tag in ("f16", "bf16"):
+        s = O.from_f32((10.0 ** rng.uniform(-7, 2, 2000)).astype(np.float32) * rng.choice([-1, 1], 2000), tag)
+        s = np.concatenate([s, O.from_f32(np.float32([1.0, 2.0 ** -20, 0.0]), tag)])
+        with np.errstate(over="ignore", invalid="ignore"):
+            got = _emulate_fnuz_stage(codes[None, :], s[:, None], tag)
+            ref = O.from_f32(O.to_f32(s, tag)[:, None] * O.round_to(w, tag)[None, :], tag)
+        gnan, rnan = np.isnan(O.to_f32(got, tag)), np.isnan(O.to_f32(ref, tag))
+        assert np.array_equal(gnan, rnan) and rnan[:, 0x80].all(), tag
+        assert np.array_equal(got[~gnan], ref[~rnan]), (tag, int(np.sum(got[~gnan] != ref[~rnan])))
