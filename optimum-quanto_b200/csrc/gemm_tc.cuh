@@ -498,7 +498,10 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
             f0 = acc[4 * j + 2 * h];
             f1 = acc[4 * j + 2 * h + 1];
           }
-          epilogue_pair<Cfg::BSRC == BSrc::TMA || Cfg::BSRC == BSrc::F8>(p, row_off, n, n + 1 < n_limit, f0, f1);
+          // int4: the output dtype is the activation dtype, so the unrolled epilogue inlines one store path per pair
+          // instead of a runtime switch over three (the int4 GEMM at M = 4096 is epilogue-bound, DESIGN section 6)
+          if constexpr (Cfg::BSRC == BSrc::INT4) epilogue_pair_t<typename Cfg::WT, false>(p, row_off, n, n + 1 < n_limit, f0, f1);
+          else epilogue_pair<Cfg::BSRC == BSrc::TMA || Cfg::BSRC == BSrc::F8>(p, row_off, n, n + 1 < n_limit, f0, f1);
         }
       }
     }
