@@ -150,6 +150,32 @@ QB200_API int qb200_qbytes_mm_quantized(const void* a, const void* w, const void
                                         const void* out_scale, int64_t m, int64_t n, int64_t k, int a_dtype, int w_dtype,
                                         int scale_dtype, int q_dtype, void* stream);
 
+/* ---- input gradient of the quantized linear (the backward's dX = gO @ W) ---------------------------------------- */
+
+/* grad_in[M, K] = grad_out[M, N] @ dequant(packed, scale, shift)[N, K] in one launch, reading the packed weights.
+ * Replaces the reference's backward composition QuantizedLinearFunction.backward (optimum/quanto/tensor/function.py:
+ * 49-63: torch.matmul(gO, other)) -> qfallback (optimum/quanto/tensor/qtensor.py: other.dequantize(), a dense [N, K] copy
+ * of the weight) -> QBitsDequantizer (optimum/quanto/tensor/qbits.py:27-49) -> a dense GEMM.
+ * The weight operand is bit-identical to qb200_dequantize_qbits; fp32 accumulation, one rounding to `dtype`, no bias.
+ * packed: canonical 4-bit storage, uint8 [N*K/group / 2, group] (as for qb200_qbits_mm with bits = 4); scale / shift
+ * [N*K/group] in `dtype` (shift: uint8 zero-points when shift_is_int); grad_out [M, N], grad_in [M, K] in `dtype`.
+ * QB200_ERR_ARG: bad shape, group not dividing K, dtype not F32 / F16 / BF16.
+ * QB200_ERR_UNSUPPORTED (the caller composes dequantize + GEMM instead): dtype F32; N % 16 != 0 (odd N included);
+ * K % 16 != 0; group neither 32 nor a multiple of 64; grad_out, packed or grad_in not 16-byte aligned.  2-bit weights
+ * have no kernel: do not pass them here. */
+QB200_API int qb200_qbits_mm_grad_input(const void* grad_out, const uint8_t* packed, const void* scale, const void* shift,
+                                        void* grad_in, int64_t m, int64_t n, int64_t k, int group, int dtype,
+                                        int shift_is_int, void* stream);
+
+/* grad_in[M, K] = grad_out[M, N] @ (scales[n] * W[n, k])[N, K] in one launch: the input gradient of the 8-bit linear.
+ * Replaces the same backward composition with QBytesDequantizer (optimum/quanto/tensor/qbytes.py:23-31: scale * data in
+ * the scale dtype, one rounding) as the dequantisation; the weight operand is bit-identical to it.
+ * W [N, K] of w_dtype in {I8, E4M3, E5M2, E4M3FNUZ}; scales [N] (one per out-feature), grad_out [M, N], grad_in [M, K]
+ * in `dtype`.  QB200_ERR_UNSUPPORTED: dtype F32; N % 8 != 0; K % 16 != 0; grad_out, W or grad_in not 16-byte aligned.
+ * A per-tensor scale has no kernel: expand it to [N] or compose. */
+QB200_API int qb200_qbytes_mm_grad_input(const void* grad_out, const void* w, const void* scales, void* grad_in,
+                                         int64_t m, int64_t n, int64_t k, int w_dtype, int dtype, void* stream);
+
 /* ---- weight freeze / calibration: the step before the hot path (SURVEY.md 8f rank 1-2) ------------------------- */
 
 /* quanto::quantize_affine(Tensor base, int bits, int axis, int? group_size, Tensor scale, Tensor shift) -> Tensor
@@ -190,7 +216,7 @@ QB200_API int qb200_absmax(const void* base, void* out, void* scratch, int64_t n
 QB200_API int qb200_quantize_qbytes_absmax(const void* base, void* out, void* scale, int64_t n, int64_t k, int dtype,
                                            int out_dtype, void* stream);
 
-/* Which kernel family the last qb200_qbytes_mm / qb200_qbits_mm call on this thread dispatched to:
+/* Which kernel family the last qb200_qbytes_mm / qb200_qbits_mm / *_grad_input call on this thread dispatched to:
  * 0 none, 1 wgmma (TMA + warpgroup MMA), 2 CUDA-core (shape-agnostic), 3 warp-MMA gemv (int4, M <= 32: TMA ring or register streaming).
  * For tests and bench accounting. */
 QB200_API int qb200_last_kernel_family(void);

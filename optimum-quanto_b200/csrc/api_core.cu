@@ -156,6 +156,24 @@ int make_tmap_2d(CUtensorMap* map, const void* base, int dt, int64_t rows, int64
   return encode_2d(map, base, dt, rows, cols, cols, 128 / esz, box_rows, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
+int make_tmap_planes(CUtensorMap* map, const void* base, int dt, int64_t rows, int64_t cols, int box_rows) {
+  EncodeTiledFn enc = get_encode_fn();
+  if (enc == nullptr) return fail(ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
+  if (dt != DT_BF16 && dt != DT_F16) return fail(ERR_ARG, "plane tensor map: 16-bit elements only");
+  if (reinterpret_cast<uintptr_t>(base) % 16 != 0) return fail(ERR_ARG, "TMA operand not 16-byte aligned");
+  if (cols % 16 != 0) return fail(ERR_ARG, "plane tensor map: cols %lld not a multiple of 16", (long long)cols);
+  const CUtensorMapDataType type = dt == DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const cuuint64_t half = static_cast<cuuint64_t>(cols / 2);
+  const cuuint64_t gdim[3] = {half, 2, static_cast<cuuint64_t>(rows)};
+  const cuuint64_t gstride[2] = {half * 2, static_cast<cuuint64_t>(cols) * 2};
+  const cuuint32_t box[3] = {64, 1, static_cast<cuuint32_t>(box_rows)};
+  const cuuint32_t estride[3] = {1, 1, 1};
+  CUresult r = enc(map, type, 3, const_cast<void*>(base), gdim, gstride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(ERR_CUDA, "cuTensorMapEncodeTiled (planes) failed with CUresult %d", static_cast<int>(r));
+  return OK;
+}
+
 int make_tmap_2d_view(CUtensorMap* map, const void* base, int dt, int64_t rows, int64_t cols, int64_t pitch_elems,
                       int box_cols, int box_rows, bool swizzle128) {
   return encode_2d(map, base, dt, rows, cols, pitch_elems, box_cols, box_rows,

@@ -181,7 +181,63 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   return d;
 }
 
+// Shared-memory matrix descriptor of an MN-major operand (imm-trans = 1: element (k, n) at row k, the MN index
+// contiguous) with the 128-byte swizzle.  A swizzle atom is 8 K-rows of 64 16-bit MN elements (128 bytes per row, chunk
+// c of row r at chunk position c ^ (r & 7)); its fields mean something else than for the K-major layout:
+//   [16,30)  leading-dim byte offset >> 4 : distance between MN atoms (MN elements 64 apart)
+//   [32,46)  stride-dim byte offset >> 4  : distance between 8-row K groups = 1024 B -> 64
+__device__ __forceinline__ uint64_t wgmma_desc_sw128_mn(uint32_t smem_addr, uint32_t mn_atom_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>((mn_atom_bytes >> 4) & 0x3FFFu) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
+  return d;
+}
+
+// 3-D tiled TMA load (coordinates innermost first)
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int32_t c0,
+                                            int32_t c1, int32_t c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
+
 enum class MmaKind { F16, BF16, I8 };
+
+// 16-bit x 16-bit -> f32, N = 128, K = 16, A K-major and B MN-major (imm-trans-b = 1, allowed for f16 / bf16 only)
+#define QB_WGMMA_ACC64_OPERANDS                                                                                   \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),      \
+      "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),       \
+      "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),      \
+      "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),      \
+      "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),      \
+      "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),      \
+      "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),      \
+      "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+#define QB_WGMMA_ACC64_LIST                                                                                          \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                          \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                                  \
+  "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                                  \
+  "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+template <MmaKind KA>
+__device__ __forceinline__ void wgmma_n128_tb(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  static_assert(KA == MmaKind::BF16 || KA == MmaKind::F16, "transposed operands are 16-bit only");
+  if constexpr (KA == MmaKind::BF16) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " QB_WGMMA_ACC64_LIST ", %64, %65, p, 1, 1, 0, 1;\n}\n"
+                 : QB_WGMMA_ACC64_OPERANDS
+                 : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+  } else {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " QB_WGMMA_ACC64_LIST ", %64, %65, p, 1, 1, 0, 1;\n}\n"
+                 : QB_WGMMA_ACC64_OPERANDS
+                 : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+  }
+}
+#undef QB_WGMMA_ACC64_OPERANDS
+#undef QB_WGMMA_ACC64_LIST
 
 
 // bf16 x bf16 -> f32, N = 128, K = 16 (32 bytes of each operand row)

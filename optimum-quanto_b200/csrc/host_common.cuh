@@ -60,6 +60,9 @@ cudaError_t launch_kernel_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 
 // Row-major [rows, cols] matrix of `dt` elements; box = 128 bytes of a row x box_rows rows, 128-byte swizzle.
 int make_tmap_2d(CUtensorMap* map, const void* base, int dt, int64_t rows, int64_t cols, int box_rows);
+// Row-major [rows, cols] 16-bit matrix described as [rows, 2, cols/2] (two column planes); box = 64 elements of one
+// plane x box_rows rows, 128-byte swizzle.  A box never crosses cols/2: past the end of a plane TMA fills zeros.
+int make_tmap_planes(CUtensorMap* map, const void* base, int dt, int64_t rows, int64_t cols, int box_rows);
 // [rows, cols] view with an explicit row pitch and box: the epilogue's TMA stores into (a column slab of) the output.
 int make_tmap_2d_view(CUtensorMap* map, const void* base, int dt, int64_t rows, int64_t cols, int64_t pitch_elems,
                       int box_cols, int box_rows, bool swizzle128);

@@ -53,6 +53,8 @@ EXPORTS = (
     "qb200_developer_build",
     "qb200_test_override",
     "qb200_qbits_ring_plan",
+    "qb200_qbits_mm_grad_input",
+    "qb200_qbytes_mm_grad_input",
 )
 
 # qb200_test_override keys (include/quanto_b200.h)
@@ -130,6 +132,8 @@ def load():
         lib.qb200_quantize_qbits_max.argtypes = [vp, vp, vp, vp, i64, i64, i32, i32, i32, i32, vp]
         lib.qb200_absmax.argtypes = [vp, vp, vp, i64, i32, vp]
         lib.qb200_quantize_qbytes_absmax.argtypes = [vp, vp, vp, i64, i64, i32, i32, vp]
+        lib.qb200_qbits_mm_grad_input.argtypes = [vp, vp, vp, vp, vp, i64, i64, i64, i32, i32, i32, vp]
+        lib.qb200_qbytes_mm_grad_input.argtypes = [vp, vp, vp, vp, i64, i64, i64, i32, i32, vp]
         for name in EXPORTS:
             getattr(lib, name)  # AttributeError here == header and library out of sync
         # Developer knock-outs exist only in a `make KNOCKOUTS=1` build and are set explicitly through

@@ -16,10 +16,12 @@ After this, every `optimum.quanto` object keeps working as before -- `quantize()
    CUDA tensors to the AWQ / TinyGemm / Marlin-FP8 repacking subclasses: the kernels read the canonical packing, so
    `create()` returns the canonical tensor and nothing is repacked at `freeze()` / `.to(device)` / load time;
 3. `F.linear(x, WeightQBitsTensor)` on CUDA calls `quanto::qbits_mm` -- ONE fused launch instead of
-   unpack + scale + shift + ungroup + matmul (tensor/weights/qbits.py:262-281, tensor/function.py:42-47); the backward is
-   the reference's own (`QuantizedLinearFunction.backward`);
+   unpack + scale + shift + ungroup + matmul (tensor/weights/qbits.py:262-281, tensor/function.py:42-47); its backward
+   takes the input gradient from `quanto::qbits_grad_input` (one launch that reads the packed weights, instead of
+   `torch.matmul(gO, other)` on a dequantised dense copy) and keeps the reference's weight and bias gradients;
 4. `WeightQBytesLinearFunction.forward` (tensor/weights/qbytes.py:68-82) keeps calling `quanto::qbytes_mm`, with the bias
-   fused into the kernel epilogue when there is one.
+   fused into the kernel epilogue when there is one; its backward takes the input gradient from
+   `quanto::qbytes_grad_input` the same way.
 
 Used by tools/run_reference_tests.py to run the reference's OWN hot-path tests (tests/library, tests/tensor/ops,
 tests/nn/test_qlinear.py) against these kernels.  Nothing here is imported by the rest of the package.
@@ -42,6 +44,7 @@ def bind_reference():
     from optimum.quanto.tensor.weights import qbytes as ref_qbytes
 
     from . import library  # noqa: F401  (re-binds the CUDA dispatch key of the shared ops, defines the fused ones)
+    from .tensor.function import linear_backward, qbits_grad_input, qbytes_grad_input
 
     RefQBits = ref_qbits.WeightQBitsTensor
     RefQBytesW = ref_qbytes.WeightQBytesTensor
@@ -75,6 +78,10 @@ def bind_reference():
             out = torch.ops.quanto.qbits_mm(input.reshape(-1, k), other._data._data, other._scale, other._shift, bias, n,
                                             group, other._qtype.bits)
             return out.reshape(input.shape[:-1] + (n,))
+
+        @staticmethod
+        def backward(ctx, gO):
+            return linear_backward(ctx, gO, qbits_grad_input)
 
     def fused_ok(w, x):
         from optimum.quanto.tensor.packed import PackedTensor
@@ -119,6 +126,10 @@ def bind_reference():
                 if bias is not None:
                     out = out + bias
             return out.reshape(input.shape[:-1] + (other.shape[0],))
+
+        @staticmethod
+        def backward(ctx, gO):
+            return linear_backward(ctx, gO, qbytes_grad_input)
 
     ref_qbytes.WeightQBytesLinearFunction = FusedQBytesLinear
     _bound = True

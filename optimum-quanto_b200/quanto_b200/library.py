@@ -11,6 +11,9 @@ adds the two fused ops that take the place of the retired AWQ / Marlin / TinyGem
   quanto::dequantize_qbits   unpack + scale + shift + ungroup in one launch
   quanto::qbytes_linear      qbytes_mm with the bias of the 8-bit linear fused into the epilogue
   quanto::qbytes_linear_quantized  ... and the per-tensor output quantisation too (quantized activations in and out)
+the input gradients of the two quantized linears (the backward's gO @ W, reading the quantized weights):
+  quanto::qbits_grad_input   packed int4 weights
+  quanto::qbytes_grad_input  int8 / float8 weights
 and the weight-freeze / calibration ops of the step before the path (SURVEY.md 8f):
   quanto::pack                    pack_weights (optimum/quanto/tensor/packed.py:24-69) as one launch
   quanto::quantize_qbits_max      MaxOptimizer + quantize_affine + pack_weights in one launch (axis 0)
@@ -64,6 +67,9 @@ _define("pack", "(Tensor self, int bits) -> Tensor")
 _define("quantize_qbits_max", "(Tensor base, int bits, int group_size, bool zeropoint) -> (Tensor, Tensor, Tensor)")
 _define("quantize_qbytes_absmax", "(Tensor base, ScalarType dtype) -> (Tensor, Tensor)")
 _define("absmax", "(Tensor base) -> Tensor")
+_define("qbits_grad_input", "(Tensor grad_output, Tensor packed, Tensor scale, Tensor shift, int out_features, "
+                            "int group_size, int bits) -> Tensor")
+_define("qbytes_grad_input", "(Tensor grad_output, Tensor B, Tensor scales) -> Tensor")
 
 
 def _require_contiguous(t: torch.Tensor, what: str) -> torch.Tensor:
@@ -437,6 +443,94 @@ def qbits_mm_cuda(activations, packed, scale, shift, bias, out_features: int, gr
     return out.reshape(activations.shape[:-1] + (out_features,))
 
 
+# ------------------------------------------------------------------------- input gradients of the linears
+def _grad_output_2d(grad_output, out_features: int, what: str):
+    if grad_output.ndim != 2 or grad_output.shape[1] != out_features:
+        raise ValueError(f"{what}: grad_output must be [M, {out_features}] (got {tuple(grad_output.shape)})")
+    return _require_contiguous(grad_output, "grad_output")
+
+
+def qbits_grad_input_cuda(grad_output, packed, scale, shift, out_features: int, group_size: int, bits: int):
+    """dX = gO @ dequant(W) for a canonical axis-0 packed weight: ONE native launch that reads the packed bytes.
+
+    Shapes the kernel declines (2-bit, fp32, N % 16 != 0, K % 16 != 0, other group sizes, unaligned buffers) run the
+    composition the reference's backward performs: dequantize (quanto::dequantize_qbits, bit-exact), then matmul."""
+    if packed.dtype != torch.uint8:
+        raise ValueError("qbits_grad_input: packed weights must be uint8")
+    if bits not in (2, 4):
+        raise ValueError("qbits_grad_input: bits must be 2 or 4")
+    gO = _grad_output_2d(grad_output, out_features, "qbits_grad_input")
+    if gO.dtype != scale.dtype:
+        raise ValueError(f"qbits_grad_input: grad_output dtype {gO.dtype} does not match the scale ({scale.dtype})")
+    if shift.dtype.is_floating_point:
+        if shift.dtype != scale.dtype:
+            raise ValueError(f"qbits_grad_input: float shift of dtype {shift.dtype} does not match the scale")
+    elif shift.dtype not in (torch.uint8, torch.int8):
+        raise ValueError("qbits_grad_input: integer shifts must be uint8 / int8 zero-points")
+    if group_size <= 0 or scale.numel() != shift.numel() or (scale.numel() * group_size) % out_features != 0:
+        raise ValueError("qbits_grad_input: scale / shift must hold one value per (out_feature, group)")
+    k = scale.numel() * group_size // out_features
+    if k % group_size != 0:
+        raise ValueError(f"qbits_grad_input: group size {group_size} does not divide in_features {k}")
+    if packed.numel() != -(-scale.numel() // (8 // bits)) * group_size:
+        raise ValueError("qbits_grad_input: packed tensor does not match out_features x in_features")
+    m = gO.shape[0]
+    packed_c = _require_contiguous(packed, "packed")
+    scale_f = _require_contiguous(scale.reshape(-1), "scale")
+    shift_f = _require_contiguous(shift.reshape(-1), "shift")
+    shift_is_int = 0 if shift_f.dtype.is_floating_point else 1
+    if shift_f.dtype == torch.int8:
+        shift_f = shift_f.view(torch.uint8)
+    if bits == 4:
+        out = torch.empty((m, k), dtype=gO.dtype, device=gO.device)
+        with torch.cuda.device(gO.device):
+            lib = N.load()
+            try:
+                N.check(lib.qb200_qbits_mm_grad_input(N.ptr(gO), N.ptr(packed_c), N.ptr(scale_f), N.ptr(shift_f),
+                                                      N.ptr(out), m, out_features, k, group_size,
+                                                      N.DTYPE_CODE[gO.dtype], shift_is_int, N.stream_ptr(gO.device)),
+                        "quanto::qbits_grad_input")
+                return out
+            except N.UnsupportedConfiguration:
+                pass
+    w = dequantize_qbits_cuda(packed, scale, shift, out_features, k, group_size, bits)
+    return torch.matmul(gO, w)
+
+
+def qbytes_grad_input_cuda(grad_output, weights, scales):
+    """dX = gO @ (scales * W) for an 8-bit weight [N, K] with per-out-feature scales: ONE native launch.
+
+    Shapes the kernel declines (fp32, per-tensor scale, N % 8 != 0, K % 16 != 0, unaligned buffers) run the composition
+    the reference's backward performs: `scales * W` in the scale dtype (QBytesDequantizer), then matmul."""
+    if weights.ndim != 2:
+        raise ValueError("qbytes_grad_input expects weights [N, K]")
+    if weights.dtype not in (torch.int8, torch.float8_e4m3fn, torch.float8_e5m2, torch.float8_e4m3fnuz):
+        raise NotImplementedError(f"qbytes_grad_input: no sm_90a kernel for weights of dtype {weights.dtype}")
+    n, k = weights.shape
+    gO = _grad_output_2d(grad_output, n, "qbytes_grad_input")
+    if gO.dtype != scales.dtype or scales.dtype not in _FLOATS:
+        raise ValueError(f"qbytes_grad_input: grad_output dtype {gO.dtype} does not match the scales ({scales.dtype})")
+    if scales.numel() == n and n > 1:
+        m = gO.shape[0]
+        w = _require_contiguous(weights, "B")
+        s = _require_contiguous(scales.reshape(-1), "scales")
+        out = torch.empty((m, k), dtype=gO.dtype, device=gO.device)
+        with torch.cuda.device(gO.device):
+            lib = N.load()
+            try:
+                N.check(lib.qb200_qbytes_mm_grad_input(N.ptr(gO), N.ptr(w), N.ptr(s), N.ptr(out), m, n, k,
+                                                       N.DTYPE_CODE[w.dtype], N.DTYPE_CODE[gO.dtype],
+                                                       N.stream_ptr(gO.device)), "quanto::qbytes_grad_input")
+                return out
+            except N.UnsupportedConfiguration:
+                pass
+    elif scales.numel() != 1:
+        raise ValueError("qbytes_grad_input: scales must have one value per output feature or one in all")
+    payload = weights.to(scales.dtype) if weights.dtype.is_floating_point else weights  # fp8 has no mul
+    scale_b = scales.reshape(-1, 1) if scales.numel() == n else scales
+    return torch.matmul(gO, scale_b * payload)
+
+
 def _bind_cuda(name: str, fn):
     """Attach the sm_90a implementation to the CUDA dispatch key, replacing the reference's CUDA binding if
     `optimum.quanto` was imported first (it registers its own for unpack / qbytes_mm,
@@ -451,6 +545,8 @@ _bind_cuda("qbytes_linear", _qbytes_linear_op)
 _bind_cuda("qbytes_linear_quantized", qbytes_linear_quantized_cuda)
 _bind_cuda("qbits_mm", qbits_mm_cuda)
 _bind_cuda("dequantize_qbits", dequantize_qbits_cuda)
+_bind_cuda("qbits_grad_input", qbits_grad_input_cuda)
+_bind_cuda("qbytes_grad_input", qbytes_grad_input_cuda)
 _bind_cuda("pack", pack_cuda)
 _bind_cuda("quantize_qbits_max", quantize_qbits_max_cuda)
 _bind_cuda("quantize_qbytes_absmax", quantize_qbytes_absmax_cuda)
