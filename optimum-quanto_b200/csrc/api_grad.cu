@@ -9,20 +9,8 @@ namespace qb {
 
 template <class Cfg>
 static int launch_dgrad(const CUtensorMap& tg, const DgradParams& p, cudaStream_t stream) {
-  int rc = ensure_dyn_smem<gemm_dgrad_kernel<Cfg>>(Cfg::SMEM_BYTES);
-  if (rc != OK) return rc;
-  const int tiles = p.num_m_blocks * p.num_k_blocks;
-  const int grid = tiles < current_sm_count() ? tiles : current_sm_count();
-  gemm_dgrad_kernel<Cfg><<<grid, Cfg::NTHREADS, Cfg::SMEM_BYTES, stream>>>(tg, p);
-  return check_cuda(cudaGetLastError(), "gemm_dgrad_kernel launch");
-}
-
-// Tile rows: 64 while M <= 64 (small batches do not pay for empty MMA rows), else 128; test override key 0 forces either.
-static int dgrad_tile_m(int64_t m) {
-  int tile_m = m <= 64 ? 64 : 128;
-  const int force_m = test_override(OVR_TILE_M);
-  if (force_m == 64 || force_m == 128) tile_m = force_m;
-  return tile_m;
+  return launch_persistent<gemm_dgrad_kernel<Cfg>, typename Cfg::Pipe>(p.num_m_blocks * p.num_k_blocks, stream,
+                                                                       "gemm_dgrad_kernel launch", tg, p);
 }
 
 static bool aligned16(const void* ptr) { return reinterpret_cast<uintptr_t>(ptr) % 16 == 0; }
@@ -78,10 +66,8 @@ static int qbits_grad_input_impl(const void* grad_out, const uint8_t* packed, co
   p.N = static_cast<int>(n);
   p.K = static_cast<int>(k);
   p.group = group;
-  p.group_log2 = -1;
-  for (int b = 0; b < 31; ++b)
-    if ((1 << b) == group) p.group_log2 = b;
-  const int tile_m = dgrad_tile_m(m);
+  p.group_log2 = group_log2(group);
+  const int tile_m = wgmma_tile_m(m);
   p.num_m_blocks = static_cast<int>((m + tile_m - 1) / tile_m);
   p.num_k_blocks = static_cast<int>((k + 127) / 128);
   p.red_blocks = static_cast<int>((n / 2 + 63) / 64);
@@ -119,7 +105,7 @@ static int qbytes_grad_input_impl(const void* grad_out, const void* w, const voi
   p.M = static_cast<int>(m);
   p.N = static_cast<int>(n);
   p.K = static_cast<int>(k);
-  const int tile_m = dgrad_tile_m(m);
+  const int tile_m = wgmma_tile_m(m);
   p.num_m_blocks = static_cast<int>((m + tile_m - 1) / tile_m);
   p.num_k_blocks = static_cast<int>((k + 127) / 128);
   p.red_blocks = static_cast<int>((n + 63) / 64);

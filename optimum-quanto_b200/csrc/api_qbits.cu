@@ -14,14 +14,10 @@ int launch_qbits_mm_simt(const void*, const uint8_t*, const void*, const void*, 
 
 template <class Cfg>
 static int launch_gemm(const CUtensorMap& ta, const GemmParams& p, cudaStream_t stream) {
-  int rc = ensure_dyn_smem<gemm_tc_kernel<Cfg>>(Cfg::SMEM_BYTES);
-  if (rc != OK) return rc;
   CUtensorMap tb;
   std::memset(&tb, 0, sizeof(tb));  // the weight tile is staged by the kernel's own warps
-  const int tiles = p.num_m_blocks * p.num_n_blocks;
-  const int grid = tiles < current_sm_count() ? tiles : current_sm_count();
-  gemm_tc_kernel<Cfg><<<grid, Cfg::NTHREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, p);
-  return check_cuda(cudaGetLastError(), "gemm_tc_kernel launch");
+  return launch_persistent<gemm_tc_kernel<Cfg>, typename Cfg::Pipe>(p.num_m_blocks * p.num_n_blocks, stream,
+                                                                    "gemm_tc_kernel launch", ta, tb, p);
 }
 
 template <int MWG>
@@ -60,9 +56,7 @@ static int qbits_mm_impl(QbitsArgs& q) {
                               static_cast<int>(k), group, q.bits, dtype, q.shift_is_int, q.ld, q.col0, q.stream);
     return rc == OK ? OK : fail(rc, "qbits_mm: CUDA-core kernel launch failed");
   }
-  q.group_log2 = -1;
-  for (int b = 0; b < 31; ++b)
-    if ((1 << b) == group) q.group_log2 = b;
+  q.group_log2 = group_log2(group);
 
   bool handled = false;
   rc = qbits_small_dispatch(q, &handled);
@@ -85,10 +79,7 @@ static int qbits_mm_impl(QbitsArgs& q) {
   p.group = group;
   p.group_log2 = q.group_log2;
   p.shift_is_int = q.shift_is_int;
-  // Tile M: one consumer warpgroup (64 rows) while M <= 64, so that small batches do not pay for empty MMA rows.
-  int tile_m = m <= 64 ? 64 : 128;
-  const int force_m = test_override(OVR_TILE_M);
-  if (force_m == 64 || force_m == 128) tile_m = force_m;
+  const int tile_m = wgmma_tile_m(m);
   constexpr int BN = 128;  // out-features per tile: 64 packed rows, both nibble planes
   p.num_m_blocks = static_cast<int>((m + tile_m - 1) / tile_m);
   p.num_n_blocks = static_cast<int>((n / 2 + BN / 2 - 1) / (BN / 2));

@@ -15,12 +15,8 @@ int launch_qbytes_mm_simt(const void*, const void*, const void*, const void*, vo
 
 template <class Cfg>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
-  int rc = ensure_dyn_smem<gemm_tc_kernel<Cfg>>(Cfg::SMEM_BYTES);
-  if (rc != OK) return rc;
-  const int tiles = p.num_m_blocks * p.num_n_blocks;
-  const int grid = tiles < current_sm_count() ? tiles : current_sm_count();
-  gemm_tc_kernel<Cfg><<<grid, Cfg::NTHREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, p);
-  return check_cuda(cudaGetLastError(), "gemm_tc_kernel launch");
+  return launch_persistent<gemm_tc_kernel<Cfg>, typename Cfg::Pipe>(p.num_m_blocks * p.num_n_blocks, stream,
+                                                                    "gemm_tc_kernel launch", ta, tb, p);
 }
 
 // Columns of tensor-core work per SM for a tile of BM x bn: waves x bn (wave quantisation included).
@@ -82,10 +78,7 @@ static int qbytes_mm_impl(const void* a, const void* w, const void* scales, cons
     p.K = static_cast<int>(k);
     return p;
   };
-  // Tile M: one consumer warpgroup (64 rows) while M <= 64, so that small batches do not pay for empty MMA rows.
-  int tile_m = m <= 64 ? 64 : 128;
-  const int force_m = test_override(OVR_TILE_M);
-  if (force_m == 64 || force_m == 128) tile_m = force_m;
+  const int tile_m = wgmma_tile_m(m);
 
   const bool both_i8 = (a_dtype == DT_I8 && w_dtype == DT_I8);
   const bool both_f8 = ((a_dtype == DT_E4M3 || a_dtype == DT_E5M2) && (w_dtype == DT_E4M3 || w_dtype == DT_E5M2));

@@ -22,6 +22,7 @@
 #include "common.cuh"
 #include "gather.cuh"
 #include "quantize_math.cuh"
+#include "wgmma_pipe.cuh"
 
 namespace qb {
 
@@ -156,18 +157,27 @@ __device__ __forceinline__ void dequant16(const uint4& raw, const typename Dq<WT
   }
 }
 
-// One nibble plane of 16 packed bytes -> 8 registers of bf16x2 / half2 (16 k of ONE out-feature, natural k order).
-template <typename WT, bool ZP>
-__device__ __forceinline__ void dequant16_plane(const uint4& raw, bool high_plane, const typename Dq<WT>::Coef& kc,
-                                                uint32_t (&o)[8]) {
-  using D = Dq<WT>;
-  const uint32_t w4[4] = {raw.x, raw.y, raw.z, raw.w};
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const uint32_t w = (high_plane ? (w4[i] >> 4) : w4[i]) & 0x0F0F0F0Fu;
-    o[2 * i + 0] = D::cvt(__byte_perm(w, D::MAGIC_BYTES, 0x4140), kc, ZP);
-    o[2 * i + 1] = D::cvt(__byte_perm(w, D::MAGIC_BYTES, 0x4342), kc, ZP);
+// The scale and shift of one group of a packed row's two out-features (low nibble: element ilo of the coefficient
+// arrays, high nibble: ihi), as 16-bit payloads: the shift is in the weight dtype, or a uint8 zero-point when ZP.
+struct CoefPair { uint16_t s_lo, s_hi, z_lo, z_hi; };
+template <bool ZP>
+__device__ __forceinline__ CoefPair load_coef_pair(const void* wscale, const void* wshift, size_t ilo, size_t ihi) {
+  CoefPair c;
+  c.s_lo = __ldg(static_cast<const uint16_t*>(wscale) + ilo);
+  c.s_hi = __ldg(static_cast<const uint16_t*>(wscale) + ihi);
+  if (ZP) {
+    c.z_lo = __ldg(static_cast<const uint8_t*>(wshift) + ilo);
+    c.z_hi = __ldg(static_cast<const uint8_t*>(wshift) + ihi);
+  } else {
+    c.z_lo = __ldg(static_cast<const uint16_t*>(wshift) + ilo);
+    c.z_hi = __ldg(static_cast<const uint16_t*>(wshift) + ihi);
   }
+  return c;
+}
+
+template <typename WT>
+__device__ __forceinline__ WT bits_as(uint16_t b) {
+  return *reinterpret_cast<const WT*>(&b);
 }
 
 // 64 packed bytes of one packed row (64 k of out-features n and n + N/2) -> two 128-byte operand rows in shared
@@ -310,20 +320,12 @@ struct GemmCfg {
   static constexpr int KBYTES = 128;    // K extent of one pipeline stage in bytes = one swizzle atom
   static constexpr int A_TILE = BM * KBYTES;
   static constexpr int B_TILE = BN * KBYTES;
-  static constexpr int STAGE = A_TILE + B_TILE;
   // staged weights: one staging group (BN/64 warps: one thread per packed int4 row, or per two 8-bit rows -- and for F8
   // per one or two activation rows) per stage slot.  3 slots keep the CTA at 15 warps, which leaves 128 registers per thread (the consumers hold 64 accumulators).
-  static constexpr int CVT_GROUP_WARPS = BN / 64;
-  static constexpr int NSTAGES = (BSRC == BSrc::TMA) ? ((192 * 1024) / STAGE > 8 ? 8 : (192 * 1024) / STAGE) : 3;
-  static constexpr int NCVT_WARPS = (BSRC == BSrc::TMA) ? 0 : NSTAGES * CVT_GROUP_WARPS;
-  static constexpr int PRODUCER_WARP = 4 * MWG;
-  static constexpr int FIRST_CVT_WARP = PRODUCER_WARP + 1;
-  static constexpr int NTHREADS = (FIRST_CVT_WARP + NCVT_WARPS) * 32;
+  static constexpr int NSTAGES =
+      (BSRC == BSrc::TMA) ? ((192 * 1024) / (A_TILE + B_TILE) > 8 ? 8 : (192 * 1024) / (A_TILE + B_TILE)) : 3;
   // the TMA producer's arrive (A tile, and W for TMA) + one per staging warp; F8 stages both operands without TMA
-  static constexpr int FULL_ARRIVALS = (BSRC == BSrc::F8 ? 0 : 1) + ((BSRC == BSrc::TMA) ? 0 : CVT_GROUP_WARPS);
-  // 1024 bytes of alignment slack (the swizzled tiles need 1024-byte aligned bases) + the barriers
-  static constexpr int SMEM_BYTES = 1024 + NSTAGES * STAGE + 2 * NSTAGES * 8;
-  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
+  using Pipe = PipeLayout<MWG, NSTAGES, A_TILE, B_TILE, (BSRC == BSrc::TMA) ? 0 : BN / 64, (BSRC == BSrc::F8) ? 0 : 1>;
   static_assert(BN == 128 || (BN == 256 && IS_INT && BSRC == BSrc::TMA), "wgmma tile width");
   static_assert(BSRC == BSrc::TMA || KIND == MmaKind::F16 || KIND == MmaKind::BF16, "staged weights are 16-bit");
 };
@@ -403,72 +405,38 @@ __device__ __forceinline__ void epilogue_pair(const GemmParams& p, size_t row_of
 // The kernel
 // ------------------------------------------------------------------------------------------------
 template <class Cfg>
-__global__ void __launch_bounds__(Cfg::NTHREADS, 1)
+__global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
     gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                    const GemmParams p) {
-  constexpr int NSTAGES = Cfg::NSTAGES;
+  using L = typename Cfg::Pipe;
   constexpr int BN = Cfg::BN;
 
-  extern __shared__ uint8_t smem_raw[];
-  // the swizzled operand tiles need 1024-byte aligned bases (SMEM_BYTES reserves the slack)
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + NSTAGES * Cfg::STAGE);
-  uint64_t* empty_bar = full_bar + NSTAGES;
+  const auto pipe = WgmmaPipe<L>::init([&] {
+    tma_prefetch_desc(&tmap_a);
+    if constexpr (Cfg::BSRC == BSrc::TMA) tma_prefetch_desc(&tmap_b);
+  });
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-
-  if (threadIdx.x == Cfg::PRODUCER_WARP * 32) {
-    tma_prefetch_desc(&tmap_a);
-    if constexpr (Cfg::BSRC == BSrc::TMA) tma_prefetch_desc(&tmap_b);
-    for (int s = 0; s < NSTAGES; ++s) {
-      mbar_init(&full_bar[s], Cfg::FULL_ARRIVALS);
-      mbar_init(&empty_bar[s], Cfg::MWG);  // one arrive per consumer warpgroup
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
 
   const int num_tiles = p.num_m_blocks * p.num_n_blocks;
   constexpr int A_ELEM = (Cfg::KIND == MmaKind::F16 || Cfg::KIND == MmaKind::BF16) ? 2 : 1;
   constexpr int KELEMS = Cfg::KBYTES / A_ELEM;  // K elements per stage
   const int kblocks = (p.K + KELEMS - 1) / KELEMS;
-  const uint32_t smem_base = smem_u32(smem);
-  auto a_addr = [&](int s) { return smem_base + s * Cfg::STAGE; };
-  auto b_addr = [&](int s) { return smem_base + s * Cfg::STAGE + Cfg::A_TILE; };
 
-  if (warp < Cfg::PRODUCER_WARP) {
+  if (warp < L::PRODUCER_WARP) {
     // ------------------------------------------------------------------ consumers: wgmma + epilogue
     const int wg = warp >> 2;
-    const bool wg_leader = (threadIdx.x & 127) == 0;
     using AccT = typename std::conditional<Cfg::IS_INT, uint32_t, float>::type;
     AccT acc[Cfg::NACC];
-    int stage = 0;
-    uint32_t phase = 0;
+    RingPos<L::NSTAGES> pos;
     const int half_n = p.N / 2;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m_blk = tile % p.num_m_blocks;
       const int n_blk = tile / p.num_m_blocks;
-      int prev = -1;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t aa = a_addr(stage) + wg * 64 * Cfg::KBYTES, bb = b_addr(stage);
-        {
-          wgmma_fence();
-          wgmma_slab<Cfg::KIND, BN>(acc, aa, bb, kb > 0);
-          wgmma_commit();
-          // keep one stage of MMAs in flight; the stage before it has been read and goes back to the producers
-          wgmma_wait<1>();
-          wgmma_fence_operands(acc);
-          if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
-          prev = stage;
-        }
-        if (++stage == NSTAGES) { stage = 0; phase ^= 1u; }
-      }
-      wgmma_wait<0>();
-      wgmma_fence_operands(acc);
-      if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
+      pipe.consume_tile(pos, kblocks, acc, [&](uint32_t aa, uint32_t bb, bool accumulate) {
+        wgmma_slab<Cfg::KIND, BN>(acc, aa, bb, accumulate);
+      });
       // epilogue straight from the fragment: thread holds rows r0 and r0 + 8, column pairs 8 j + 2 (lane % 4)
       const int r0 = m_blk * Cfg::BM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
@@ -506,233 +474,159 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
       }
     }
     if (p.g.n_out > 1) __threadfence_system();  // this thread's peer stores are performed before the rank signals
-  } else if (warp == Cfg::PRODUCER_WARP) {
+  } else if (warp == L::PRODUCER_WARP) {
     // ------------------------------------------------------------------ TMA producer
     if (lane == 0 && Cfg::BSRC != BSrc::F8) {
-      int stage = 0;
-      uint32_t phase = 0;
       constexpr uint32_t tx_bytes = Cfg::A_TILE + (Cfg::BSRC == BSrc::TMA ? Cfg::B_TILE : 0);
       gather_wait_start(p.g);  // the activation may be the gathered output of the previous linear
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile % p.num_m_blocks;
-        const int n_blk = tile / p.num_m_blocks;
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
-          tma_load_2d(smem + stage * Cfg::STAGE, &tmap_a, &full_bar[stage], kb * KELEMS, m_blk * Cfg::BM);
-          if constexpr (Cfg::BSRC == BSrc::TMA)
-            tma_load_2d(smem + stage * Cfg::STAGE + Cfg::A_TILE, &tmap_b, &full_bar[stage], kb * KELEMS, n_blk * BN);
-          if (++stage == NSTAGES) { stage = 0; phase ^= 1u; }
+      pipe.produce(num_tiles, p.num_m_blocks, kblocks, tx_bytes, [&](uint8_t* dst, uint64_t* bar, int m_blk, int n_blk, int kb) {
+        tma_load_2d(dst, &tmap_a, bar, kb * KELEMS, m_blk * Cfg::BM);
+        if constexpr (Cfg::BSRC == BSrc::TMA) tma_load_2d(dst + Cfg::A_TILE, &tmap_b, bar, kb * KELEMS, n_blk * BN);
+      });
+    }
+  } else if constexpr (Cfg::BSRC == BSrc::INT4) {
+    // ------------------------------------------------------------------ weight staging: int4 -> WT tile
+    StagingThread<L> sg(pipe, num_tiles, kblocks);
+    const int r = sg.r;
+    const uint32_t sw = static_cast<uint32_t>(r) & 7;
+    using WT = typename Cfg::WT;
+    using D = Dq<WT>;
+    constexpr bool ZP = Cfg::ZP;
+    constexpr int ROWP = BN / 2;  // packed rows per tile, one per thread of the group
+    static_assert(ROWP == StagingThread<L>::GT, "one staging thread per packed row");
+    const int half_n = p.N / 2;
+    const int groups_per_row = p.K / p.group;
+    const bool two_sets = p.group < 64;  // group size 32: two (scale, shift) pairs per 64-k stage
+
+    struct Pre {
+      uint4 raw[4];
+      WT s_lo[2], s_hi[2];
+      uint16_t z_lo[2], z_hi[2];
+      bool ok;
+    };
+    auto load_pre = [&](Pre& pr, const StageSeq<L::NSTAGES>& seq) {
+      const int rp = (seq.tile / p.num_m_blocks) * ROWP + r;
+      const int kbase = seq.kb * 64;
+      pr.ok = rp < half_n && kbase < p.K;
+      if (pr.ok) {
+        const uint8_t* src = p.wq + static_cast<size_t>(rp) * p.K + kbase;
+#pragma unroll
+        for (int v = 0; v < 4; ++v)
+          pr.raw[v] = (kbase + v * 16 < p.K) ? __ldg(reinterpret_cast<const uint4*>(src + v * 16)) : make_uint4(0, 0, 0, 0);
+        const int g0 = (p.group_log2 >= 0) ? (kbase >> p.group_log2) : (kbase / p.group);
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          if (s == 1 && !two_sets) break;
+          if (s == 1 && kbase + 32 >= p.K) {
+            // K tail (K % 64 == 32 with groups of 32): the second half of the stage lies beyond K -- its activations are
+            // zero-filled, but its coefficients would be read past the row (past the ARRAY for the last row: NaN bits
+            // there turn 0 * w into NaN)
+            pr.s_lo[1] = pr.s_lo[0]; pr.s_hi[1] = pr.s_hi[0]; pr.z_lo[1] = pr.z_lo[0]; pr.z_hi[1] = pr.z_hi[0];
+            break;
+          }
+          const size_t ilo = static_cast<size_t>(rp) * groups_per_row + g0 + s;
+          const size_t ihi = ilo + static_cast<size_t>(half_n) * groups_per_row;
+          const CoefPair c = load_coef_pair<ZP>(p.wscale, p.wshift, ilo, ihi);
+          pr.s_lo[s] = bits_as<WT>(c.s_lo);
+          pr.s_hi[s] = bits_as<WT>(c.s_hi);
+          pr.z_lo[s] = c.z_lo;
+          pr.z_hi[s] = c.z_hi;
         }
       }
-    }
-  } else {
-    // ------------------------------------------------------------------ weight staging (int4 / 8-bit -> WT tile)
-    const int ct = threadIdx.x - Cfg::FIRST_CVT_WARP * 32;
-    constexpr int GT = Cfg::CVT_GROUP_WARPS * 32;  // threads per staging group
-    const int grp = ct / GT;                         // staging group == pipeline slot it owns
-    const int r = ct % GT;
-    const int my_tiles = (num_tiles > static_cast<int>(blockIdx.x))
-                             ? (num_tiles - 1 - static_cast<int>(blockIdx.x)) / static_cast<int>(gridDim.x) + 1
-                             : 0;
-    const int total_it = my_tiles * kblocks;
-    const uint32_t bt = b_addr(grp);  // this group's B tile
-    const uint32_t full_addr = smem_u32(full_bar) + grp * 8, empty_addr = smem_u32(empty_bar) + grp * 8;
-    const uint32_t sw = static_cast<uint32_t>(r) & 7;
-    if constexpr (Cfg::BSRC == BSrc::INT4) {
-      using WT = typename Cfg::WT;
-      using D = Dq<WT>;
-      constexpr bool ZP = Cfg::ZP;
-      constexpr int ROWP = BN / 2;  // packed rows per tile, one per thread of the group
-      static_assert(ROWP == GT, "one staging thread per packed row");
-      const int half_n = p.N / 2;
-      const int groups_per_row = p.K / p.group;
-      const bool two_sets = p.group < 64;  // group size 32: two (scale, shift) pairs per 64-k stage
-      const WT* scale = static_cast<const WT*>(p.wscale);
+    };
 
-      // This group's stage sequence: it = grp, grp + NSTAGES, ...   (tile, kb) advance incrementally.
-      struct Pre {
-        uint4 raw[4];
-        WT s_lo[2], s_hi[2];
-        uint16_t z_lo[2], z_hi[2];
-        bool ok;
-      };
-      int f_it = grp;
-      int f_kb = grp % kblocks;
-      int f_tile = blockIdx.x + (grp / kblocks) * gridDim.x;
-      auto load_pre = [&](Pre& pr) {
-        if (f_it >= total_it) return;
-        const int rp = (f_tile / p.num_m_blocks) * ROWP + r;
-        const int kbase = f_kb * 64;
-        pr.ok = rp < half_n && kbase < p.K;
-        if (pr.ok) {
-          const uint8_t* src = p.wq + static_cast<size_t>(rp) * p.K + kbase;
+    const uint32_t off_lo = (static_cast<uint32_t>(r) >> 3) * 1024 + (static_cast<uint32_t>(r) & 7) * 128;
+    const uint32_t off_hi = off_lo + (ROWP / 8) * 1024;
+    sg.template run_ping_pong<Pre>(load_pre, [&](const Pre& cur) {
+      sg.wait_empty();
+      if (cur.ok) {
+        typename D::Coef klo[2], khi[2];
+        klo[0] = D::make_raw(cur.s_lo[0], cur.z_lo[0], ZP);
+        khi[0] = D::make_raw(cur.s_hi[0], cur.z_hi[0], ZP);
+        if (two_sets) {
+          klo[1] = D::make_raw(cur.s_lo[1], cur.z_lo[1], ZP);
+          khi[1] = D::make_raw(cur.s_hi[1], cur.z_hi[1], ZP);
+        } else {
+          klo[1] = klo[0];
+          khi[1] = khi[0];
+        }
+        stage_rowpair_64k<WT, ZP>(cur.raw, klo, khi, sg.bt + off_lo, sg.bt + off_hi, sw);
+      } else {
+        zero_rowpair_64k(sg.bt + off_lo, sg.bt + off_hi);
+      }
+      sg.publish();
+    });
+  } else if constexpr (Cfg::BSRC == BSrc::BYTES || Cfg::BSRC == BSrc::F8) {
+    // ------------------------------------------------------------------ weight staging: 8-bit weights (int8 / fp8) ->
+    // activation dtype, scale pre-applied (reference rounding order); F8: the weights unscaled (the scale is applied to
+    // the fp32 result) and the activation rows of the tile as well
+    StagingThread<L> sg(pipe, num_tiles, kblocks);
+    constexpr int GT = StagingThread<L>::GT;
+    const int r = sg.r;
+    const uint32_t sw = static_cast<uint32_t>(r) & 7;
+    using WT = typename Cfg::WT;
+    static_assert(GT == BN / 2, "thread r converts weight rows r and r + BN/2");
+    const WT* scale = static_cast<const WT*>(p.wscale);
+    struct PreB {
+      uint4 raw0[4], raw1[4];
+    };
+    auto load_pre = [&](PreB& pr, const StageSeq<L::NSTAGES>& seq) {
+      const int n0 = (seq.tile / p.num_m_blocks) * BN + r;
+      const int n1 = n0 + GT;
+      const int kbase = seq.kb * 64;
+#pragma unroll
+      for (int v = 0; v < 4; ++v) {
+        const bool kok = kbase + v * 16 < p.K;
+        pr.raw0[v] = (n0 < p.N && kok) ? __ldg(reinterpret_cast<const uint4*>(p.wq + static_cast<size_t>(n0) * p.K + kbase) + v)
+                                       : make_uint4(0, 0, 0, 0);
+        pr.raw1[v] = (n1 < p.N && kok) ? __ldg(reinterpret_cast<const uint4*>(p.wq + static_cast<size_t>(n1) * p.K + kbase) + v)
+                                       : make_uint4(0, 0, 0, 0);
+      }
+    };
+    const uint32_t off0 = (static_cast<uint32_t>(r) >> 3) * 1024 + (static_cast<uint32_t>(r) & 7) * 128;
+    const uint32_t off1 = off0 + (GT / 8) * 1024;
+    int c_tile = -1;
+    uint32_t s2_0 = 0, s2_1 = 0;
+    auto process = [&](const PreB& cur, const StageSeq<L::NSTAGES>& seq) {
+      if (Cfg::BSRC == BSrc::F8) {
+        s2_0 = s2_1 = 0x3F803F80u;  // bf16 1.0 pair: the conversion alone, exact
+      } else if (seq.tile != c_tile) {  // new tile: (re)load the two per-row scales (zero rows beyond N contribute exact zeros)
+        c_tile = seq.tile;
+        const int n0 = (c_tile / p.num_m_blocks) * BN + r;
+        const int n1 = n0 + GT;
+        const WT z = from_float<WT>(0.f);
+        const WT a = (n0 < p.N) ? scale[n0] : z, b = (n1 < p.N) ? scale[n1] : z;
+        const uint16_t ab = *reinterpret_cast<const uint16_t*>(&a), bb = *reinterpret_cast<const uint16_t*>(&b);
+        s2_0 = static_cast<uint32_t>(ab) * 0x00010001u;
+        s2_1 = static_cast<uint32_t>(bb) * 0x00010001u;
+      }
+      sg.wait_empty();
+      stage_row_64k<WT, Cfg::WKIND>(cur.raw0, s2_0, sg.bt + off0, sw);
+      stage_row_64k<WT, Cfg::WKIND>(cur.raw1, s2_1, sg.bt + off1, sw);
+      if constexpr (Cfg::BSRC == BSrc::F8) {
+        // activation rows r and r + 64 of the tile (BM = 64 or 128), loaded here rather than prefetched: the staging
+        // thread has no registers left for a second pair of ping-pong buffers
+        const int kbase = seq.kb * 64;
+        const uint32_t at = sg.bt - Cfg::A_TILE;
+#pragma unroll
+        for (int h = 0; h < Cfg::BM / 64; ++h) {
+          const int ar = r + 64 * h;
+          const int m = (seq.tile % p.num_m_blocks) * Cfg::BM + ar;
+          uint4 raw[4];
 #pragma unroll
           for (int v = 0; v < 4; ++v)
-            pr.raw[v] = (kbase + v * 16 < p.K) ? __ldg(reinterpret_cast<const uint4*>(src + v * 16)) : make_uint4(0, 0, 0, 0);
-          const int g0 = (p.group_log2 >= 0) ? (kbase >> p.group_log2) : (kbase / p.group);
-#pragma unroll
-          for (int st = 0; st < 2; ++st) {
-            if (st == 1 && !two_sets) break;
-            if (st == 1 && kbase + 32 >= p.K) {
-              // K tail (K % 64 == 32 with groups of 32): the second half of the stage lies beyond K -- its activations are
-              // zero-filled, but its coefficients would be read past the row (past the ARRAY for the last row: NaN bits
-              // there turn 0 * w into NaN)
-              pr.s_lo[1] = pr.s_lo[0]; pr.s_hi[1] = pr.s_hi[0]; pr.z_lo[1] = pr.z_lo[0]; pr.z_hi[1] = pr.z_hi[0];
-              break;
-            }
-            const size_t ilo = static_cast<size_t>(rp) * groups_per_row + g0 + st;
-            const size_t ihi = ilo + static_cast<size_t>(half_n) * groups_per_row;
-            pr.s_lo[st] = __ldg(scale + ilo);
-            pr.s_hi[st] = __ldg(scale + ihi);
-            if (ZP) {
-              pr.z_lo[st] = __ldg(static_cast<const uint8_t*>(p.wshift) + ilo);
-              pr.z_hi[st] = __ldg(static_cast<const uint8_t*>(p.wshift) + ihi);
-            } else {
-              pr.z_lo[st] = __ldg(static_cast<const uint16_t*>(p.wshift) + ilo);
-              pr.z_hi[st] = __ldg(static_cast<const uint16_t*>(p.wshift) + ihi);
-            }
-          }
-        }
-        f_it += NSTAGES;
-        f_kb += NSTAGES;
-        while (f_kb >= kblocks) { f_kb -= kblocks; f_tile += gridDim.x; }
-      };
-
-      const uint32_t off_lo = (static_cast<uint32_t>(r) >> 3) * 1024 + (static_cast<uint32_t>(r) & 7) * 128;
-      const uint32_t off_hi = off_lo + (ROWP / 8) * 1024;
-      uint32_t phase = 0;
-      auto process = [&](const Pre& cur) {
-        mbar_wait_u32(empty_addr, phase ^ 1u);
-        if (cur.ok) {
-          typename D::Coef klo[2], khi[2];
-          klo[0] = D::make_raw(cur.s_lo[0], cur.z_lo[0], ZP);
-          khi[0] = D::make_raw(cur.s_hi[0], cur.z_hi[0], ZP);
-          if (two_sets) {
-            klo[1] = D::make_raw(cur.s_lo[1], cur.z_lo[1], ZP);
-            khi[1] = D::make_raw(cur.s_hi[1], cur.z_hi[1], ZP);
-          } else {
-            klo[1] = klo[0];
-            khi[1] = khi[0];
-          }
-          stage_rowpair_64k<WT, ZP>(cur.raw, klo, khi, bt + off_lo, bt + off_hi, sw);
-        } else {
-          zero_rowpair_64k(bt + off_lo, bt + off_hi);
-        }
-        fence_proxy_async_smem();  // every writer: generic-proxy stores -> visible to the async proxy
-        __syncwarp();
-        if (lane == 0) mbar_arrive_u32(full_addr);  // one arrive per warp
-        phase ^= 1u;
-      };
-      // Ping-pong prefetch buffers (no register copies: copying a register that a load is still filling would
-      // stall on the load).  The group's next stage is NSTAGES pipeline stages ahead: ample time to cover L2 latency.
-      Pre pa, pb;
-      load_pre(pa);
-      for (int it = grp; it < total_it; it += 2 * NSTAGES) {
-        load_pre(pb);
-        process(pa);
-        if (it + NSTAGES < total_it) {
-          load_pre(pa);
-          process(pb);
+            raw[v] = (m < p.M && kbase + v * 16 < p.K)
+                         ? __ldg(reinterpret_cast<const uint4*>(static_cast<const uint8_t*>(p.a) + static_cast<size_t>(m) * p.K + kbase) + v)
+                         : make_uint4(0, 0, 0, 0);
+          const uint32_t aoff = (static_cast<uint32_t>(ar) >> 3) * 1024 + (static_cast<uint32_t>(ar) & 7) * 128;
+          stage_row_64k<WT, Cfg::AKIND>(raw, 0x3F803F80u, at + aoff, sw);
         }
       }
-    }
-    if constexpr (Cfg::BSRC == BSrc::BYTES || Cfg::BSRC == BSrc::F8) {
-      // ---------------- 8-bit weights (int8 / fp8) -> activation dtype, scale pre-applied (reference rounding order);
-      // F8: the weights unscaled (the scale is applied to the fp32 result) and the activation rows of the tile as well
-      using WT = typename Cfg::WT;
-      static_assert(GT == BN / 2, "thread r converts weight rows r and r + BN/2");
-      const WT* scale = static_cast<const WT*>(p.wscale);
-      struct PreB {
-        uint4 raw0[4], raw1[4];
-      };
-      int f_it = grp;
-      int f_kb = grp % kblocks;
-      int f_tile = blockIdx.x + (grp / kblocks) * gridDim.x;
-      auto load_pre = [&](PreB& pr) {
-        if (f_it >= total_it) return;
-        const int n0 = (f_tile / p.num_m_blocks) * BN + r;
-        const int n1 = n0 + GT;
-        const int kbase = f_kb * 64;
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          const bool kok = kbase + v * 16 < p.K;
-          pr.raw0[v] = (n0 < p.N && kok) ? __ldg(reinterpret_cast<const uint4*>(p.wq + static_cast<size_t>(n0) * p.K + kbase) + v)
-                                         : make_uint4(0, 0, 0, 0);
-          pr.raw1[v] = (n1 < p.N && kok) ? __ldg(reinterpret_cast<const uint4*>(p.wq + static_cast<size_t>(n1) * p.K + kbase) + v)
-                                         : make_uint4(0, 0, 0, 0);
-        }
-        f_it += NSTAGES;
-        f_kb += NSTAGES;
-        while (f_kb >= kblocks) { f_kb -= kblocks; f_tile += gridDim.x; }
-      };
-      const uint32_t off0 = (static_cast<uint32_t>(r) >> 3) * 1024 + (static_cast<uint32_t>(r) & 7) * 128;
-      const uint32_t off1 = off0 + (GT / 8) * 1024;
-      uint32_t phase = 0;
-      int c_tile = -1, c_kb = grp % kblocks, c_t = blockIdx.x + (grp / kblocks) * gridDim.x;
-      uint32_t s2_0 = 0, s2_1 = 0;
-      auto process = [&](const PreB& cur) {
-        if (Cfg::BSRC == BSrc::F8) {
-          s2_0 = s2_1 = 0x3F803F80u;  // bf16 1.0 pair: the conversion alone, exact
-        } else if (c_t != c_tile) {  // new tile: (re)load the two per-row scales (zero rows beyond N contribute exact zeros)
-          c_tile = c_t;
-          const int n0 = (c_t / p.num_m_blocks) * BN + r;
-          const int n1 = n0 + GT;
-          const WT z = from_float<WT>(0.f);
-          const WT a = (n0 < p.N) ? scale[n0] : z, b = (n1 < p.N) ? scale[n1] : z;
-          const uint16_t ab = *reinterpret_cast<const uint16_t*>(&a), bb = *reinterpret_cast<const uint16_t*>(&b);
-          s2_0 = static_cast<uint32_t>(ab) * 0x00010001u;
-          s2_1 = static_cast<uint32_t>(bb) * 0x00010001u;
-        }
-        mbar_wait_u32(empty_addr, phase ^ 1u);
-        stage_row_64k<WT, Cfg::WKIND>(cur.raw0, s2_0, bt + off0, sw);
-        stage_row_64k<WT, Cfg::WKIND>(cur.raw1, s2_1, bt + off1, sw);
-        if constexpr (Cfg::BSRC == BSrc::F8) {
-          // activation rows r and r + 64 of the tile (BM = 64 or 128), loaded here rather than prefetched: the staging
-          // thread has no registers left for a second pair of ping-pong buffers
-          const int kbase = c_kb * 64;
-          const uint32_t at = bt - Cfg::A_TILE;
-#pragma unroll
-          for (int h = 0; h < Cfg::BM / 64; ++h) {
-            const int ar = r + 64 * h;
-            const int m = (c_t % p.num_m_blocks) * Cfg::BM + ar;
-            uint4 raw[4];
-#pragma unroll
-            for (int v = 0; v < 4; ++v)
-              raw[v] = (m < p.M && kbase + v * 16 < p.K)
-                           ? __ldg(reinterpret_cast<const uint4*>(static_cast<const uint8_t*>(p.a) + static_cast<size_t>(m) * p.K + kbase) + v)
-                           : make_uint4(0, 0, 0, 0);
-            const uint32_t aoff = (static_cast<uint32_t>(ar) >> 3) * 1024 + (static_cast<uint32_t>(ar) & 7) * 128;
-            stage_row_64k<WT, Cfg::AKIND>(raw, 0x3F803F80u, at + aoff, sw);
-          }
-        }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_u32(full_addr);
-        phase ^= 1u;
-        c_kb += NSTAGES;
-        while (c_kb >= kblocks) { c_kb -= kblocks; c_t += gridDim.x; }
-      };
-      if constexpr (Cfg::BSRC == BSrc::F8) {
-        // one stage in registers at a time: the activation rows of the stage need the registers of a second buffer
-        for (int it = grp; it < total_it; it += NSTAGES) {
-          PreB pa;
-          load_pre(pa);
-          process(pa);
-        }
-      } else {
-        PreB pa, pb;
-        load_pre(pa);
-        for (int it = grp; it < total_it; it += 2 * NSTAGES) {
-          load_pre(pb);
-          process(pa);
-          if (it + NSTAGES < total_it) {
-            load_pre(pa);
-            process(pb);
-          }
-        }
-      }
-    }
+      sg.publish();
+    };
+    // F8: one stage in registers at a time, the activation rows of the stage need the registers of a second buffer
+    if constexpr (Cfg::BSRC == BSrc::F8) sg.template run_single<PreB>(load_pre, process);
+    else sg.template run_ping_pong<PreB>(load_pre, process);
   }
 
   __syncthreads();

@@ -3,7 +3,7 @@
 //   dX[m, k] = sum_n gO[m, n] * dequant(W)[n, k]
 //
 // One CTA per SM loops over BM x 128 tiles of dX (BM = 64 per consumer warpgroup); the columns of a tile are the weight's
-// in-features k and the reduction runs over its out-features n.  Roles, as in gemm_tc_kernel:
+// in-features k and the reduction runs over its out-features n.  The pipeline is the forward's (wgmma_pipe.cuh); roles:
 //   warps [0, 4*MWG)  consumers    : wgmma with fp32 accumulators in registers, then one rounding to the gradient dtype
 //   warp 4*MWG        TMA producer : the gO tiles
 //   further warps     staging      : read the packed int4 (or 8-bit) weight bytes, dequantise them with the forward's exact
@@ -53,87 +53,43 @@ struct DgradCfg {
   static constexpr int A_TILE = (INT4 ? 2 : 1) * A_PLANE;
   static constexpr int B_ATOM = RED * 128;              // 64 k columns of every reduction row of the stage
   static constexpr int B_TILE = 2 * B_ATOM;
-  static constexpr int STAGE = A_TILE + B_TILE;
   static constexpr int NSTAGES = 3;
-  static constexpr int CVT_GROUP_WARPS = 2;             // 64 staging threads: one packed (or 8-bit) row each
-  static constexpr int NCVT_WARPS = NSTAGES * CVT_GROUP_WARPS;
-  static constexpr int PRODUCER_WARP = 4 * MWG;
-  static constexpr int FIRST_CVT_WARP = PRODUCER_WARP + 1;
-  static constexpr int NTHREADS = (FIRST_CVT_WARP + NCVT_WARPS) * 32;
-  static constexpr int FULL_ARRIVALS = 1 + CVT_GROUP_WARPS;
-  static constexpr int SMEM_BYTES = 1024 + NSTAGES * STAGE + 2 * NSTAGES * 8;
-  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
+  // 64 staging threads per slot: one packed (or 8-bit) row each; the TMA producer's arrive for gO
+  using Pipe = PipeLayout<MWG, NSTAGES, A_TILE, B_TILE, 2, 1>;
 };
 
-template <typename WT>
-__device__ __forceinline__ WT bits_as(uint16_t b) {
-  return *reinterpret_cast<const WT*>(&b);
-}
-
 template <class Cfg>
-__global__ void __launch_bounds__(Cfg::NTHREADS, 1)
+__global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
     gemm_dgrad_kernel(const __grid_constant__ CUtensorMap tmap_g, const DgradParams p) {
-  constexpr int NSTAGES = Cfg::NSTAGES;
+  using L = typename Cfg::Pipe;
   using WT = typename Cfg::WT;
 
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + NSTAGES * Cfg::STAGE);
-  uint64_t* empty_bar = full_bar + NSTAGES;
+  const auto pipe = WgmmaPipe<L>::init([&] { tma_prefetch_desc(&tmap_g); });
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (threadIdx.x == Cfg::PRODUCER_WARP * 32) {
-    tma_prefetch_desc(&tmap_g);
-    for (int s = 0; s < NSTAGES; ++s) {
-      mbar_init(&full_bar[s], Cfg::FULL_ARRIVALS);
-      mbar_init(&empty_bar[s], Cfg::MWG);
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-
   const int num_tiles = p.num_m_blocks * p.num_k_blocks;
   const int kblocks = p.red_blocks;
-  const uint32_t smem_base = smem_u32(smem);
-  auto a_addr = [&](int s) { return smem_base + s * Cfg::STAGE; };
-  auto b_addr = [&](int s) { return smem_base + s * Cfg::STAGE + Cfg::A_TILE; };
 
-  if (warp < Cfg::PRODUCER_WARP) {
+  if (warp < L::PRODUCER_WARP) {
     // ------------------------------------------------------------------ consumers: wgmma + epilogue
     const int wg = warp >> 2;
-    const bool wg_leader = (threadIdx.x & 127) == 0;
     float acc[64];
-    int stage = 0;
-    uint32_t phase = 0;
+    RingPos<L::NSTAGES> pos;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m_blk = tile % p.num_m_blocks;
       const int k_blk = tile / p.num_m_blocks;
-      int prev = -1;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t aa = a_addr(stage) + wg * 64 * 128, bb = b_addr(stage);
-        wgmma_fence();
+      pipe.consume_tile(pos, kblocks, acc, [&](uint32_t aa, uint32_t bb, bool accumulate) {
 #pragma unroll
         for (int s = 0; s < Cfg::RED / 16; ++s) {
           // int4: steps 0..3 reduce the low-nibble plane (A box 0), steps 4..7 the high-nibble plane (A box 1)
           const uint32_t a_s = aa + (s / 4) * Cfg::A_PLANE + (s % 4) * 32;
           const uint32_t b_s = bb + s * 2048;  // 16 reduction rows = two 8-row groups
           wgmma_n128_tb<Cfg::KIND>(acc, wgmma_desc_sw128(a_s), wgmma_desc_sw128_mn(b_s, Cfg::B_ATOM),
-                                   (s > 0 || kb > 0) ? 1u : 0u);
+                                   (s > 0 || accumulate) ? 1u : 0u);
         }
-        wgmma_commit();
-        wgmma_wait<1>();
-        wgmma_fence_operands(acc);
-        if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
-        prev = stage;
-        if (++stage == NSTAGES) { stage = 0; phase ^= 1u; }
-      }
-      wgmma_wait<0>();
-      wgmma_fence_operands(acc);
-      if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
+      });
       // fragment: thread holds rows r0 and r0 + 8, column pairs 8 j + 2 (lane % 4); K % 16 == 0, so a pair is whole
       const int r0 = m_blk * Cfg::BM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
       WT* out = static_cast<WT*>(p.out);
@@ -150,55 +106,24 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
         }
       }
     }
-  } else if (warp == Cfg::PRODUCER_WARP) {
+  } else if (warp == L::PRODUCER_WARP) {
     // ------------------------------------------------------------------ TMA producer (gO)
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile % p.num_m_blocks;
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          mbar_arrive_expect_tx(&full_bar[stage], Cfg::A_TILE);
-          uint8_t* dst = smem + stage * Cfg::STAGE;
-          if constexpr (Cfg::INT4) {
-            tma_load_3d(dst, &tmap_g, &full_bar[stage], kb * 64, 0, m_blk * Cfg::BM);
-            tma_load_3d(dst + Cfg::A_PLANE, &tmap_g, &full_bar[stage], kb * 64, 1, m_blk * Cfg::BM);
-          } else {
-            tma_load_2d(dst, &tmap_g, &full_bar[stage], kb * 64, m_blk * Cfg::BM);
-          }
-          if (++stage == NSTAGES) { stage = 0; phase ^= 1u; }
+      pipe.produce(num_tiles, p.num_m_blocks, kblocks, Cfg::A_TILE, [&](uint8_t* dst, uint64_t* bar, int m_blk, int, int kb) {
+        if constexpr (Cfg::INT4) {
+          tma_load_3d(dst, &tmap_g, bar, kb * 64, 0, m_blk * Cfg::BM);
+          tma_load_3d(dst + Cfg::A_PLANE, &tmap_g, bar, kb * 64, 1, m_blk * Cfg::BM);
+        } else {
+          tma_load_2d(dst, &tmap_g, bar, kb * 64, m_blk * Cfg::BM);
         }
-      }
+      });
     }
   } else {
     // ------------------------------------------------------------------ weight staging
-    const int ct = threadIdx.x - Cfg::FIRST_CVT_WARP * 32;
-    const int grp = ct / 64;  // staging group == pipeline slot it owns
-    const int r = ct % 64;
-    const int my_tiles = (num_tiles > static_cast<int>(blockIdx.x))
-                             ? (num_tiles - 1 - static_cast<int>(blockIdx.x)) / static_cast<int>(gridDim.x) + 1
-                             : 0;
-    const int total_it = my_tiles * kblocks;
-    const uint32_t bt = b_addr(grp);
-    const uint32_t full_addr = smem_u32(full_bar) + grp * 8, empty_addr = smem_u32(empty_bar) + grp * 8;
+    StagingThread<L> sg(pipe, num_tiles, kblocks);
+    const int r = sg.r;
     const uint32_t sw = static_cast<uint32_t>(r) & 7;
     const uint32_t off_r = (static_cast<uint32_t>(r) >> 3) * 1024 + (static_cast<uint32_t>(r) & 7) * 128;
-    int f_it = grp;
-    int f_kb = grp % kblocks;
-    int f_tile = blockIdx.x + (grp / kblocks) * gridDim.x;
-    auto advance = [&]() {
-      f_it += NSTAGES;
-      f_kb += NSTAGES;
-      while (f_kb >= kblocks) { f_kb -= kblocks; f_tile += gridDim.x; }
-    };
-    uint32_t phase = 0;
-    auto publish = [&]() {
-      fence_proxy_async_smem();  // generic-proxy stores -> visible to the async proxy (wgmma)
-      __syncwarp();
-      if (lane == 0) mbar_arrive_u32(full_addr);
-      phase ^= 1u;
-    };
 
     if constexpr (Cfg::INT4) {
       using D = Dq<WT>;
@@ -211,12 +136,11 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
         uint4 raw[8];
         uint32_t s[4], z[4];  // low plane in bits [0, 16), high plane in [16, 32)
         int k0, g0;
-        bool ok;
+        bool ok = false;
       };
-      auto load_pre = [&](Pre& pr) {
-        if (f_it >= total_it) return;
-        const int rp = f_kb * 64 + r;
-        const int k0 = (f_tile / p.num_m_blocks) * 128;
+      auto load_pre = [&](Pre& pr, const StageSeq<L::NSTAGES>& seq) {
+        const int rp = seq.kb * 64 + r;
+        const int k0 = (seq.tile / p.num_m_blocks) * 128;
         pr.k0 = k0;
         pr.ok = rp < half_n;
         if (pr.ok) {
@@ -232,24 +156,14 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
           for (int st = 0; st < 4; ++st) {
             if (st > 1 && p.group >= 64) break;  // groups of 64 or more span at most two sets of a 128-k stage
             const int g = min(g0 + st, gpr - 1);
-            uint32_t slo, shi, zlo, zhi;
-            slo = __ldg(static_cast<const uint16_t*>(p.wscale) + row_lo + g);
-            shi = __ldg(static_cast<const uint16_t*>(p.wscale) + row_hi + g);
-            if (ZP) {
-              zlo = __ldg(static_cast<const uint8_t*>(p.wshift) + row_lo + g);
-              zhi = __ldg(static_cast<const uint8_t*>(p.wshift) + row_hi + g);
-            } else {
-              zlo = __ldg(static_cast<const uint16_t*>(p.wshift) + row_lo + g);
-              zhi = __ldg(static_cast<const uint16_t*>(p.wshift) + row_hi + g);
-            }
-            pr.s[st] = slo | (shi << 16);
-            pr.z[st] = zlo | (zhi << 16);
+            const CoefPair c = load_coef_pair<ZP>(p.wscale, p.wshift, row_lo + g, row_hi + g);
+            pr.s[st] = c.s_lo | (static_cast<uint32_t>(c.s_hi) << 16);
+            pr.z[st] = c.z_lo | (static_cast<uint32_t>(c.z_hi) << 16);
           }
         }
-        advance();
       };
-      auto process = [&](const Pre& cur) {
-        mbar_wait_u32(empty_addr, phase ^ 1u);
+      sg.template run_ping_pong<Pre>(load_pre, [&](const Pre& cur) {
+        sg.wait_empty();
         if (cur.ok) {
 #pragma unroll
           for (int v = 0; v < 8; ++v) {
@@ -266,7 +180,7 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
                                                      static_cast<uint16_t>(z >> 16), ZP);
             uint32_t lo[8], hi[8];
             dequant16<WT, ZP>(cur.raw[v], klo, khi, lo, hi);
-            const uint32_t atom = bt + (v / 4) * Cfg::B_ATOM + off_r;
+            const uint32_t atom = sg.bt + (v / 4) * Cfg::B_ATOM + off_r;
             const uint32_t c0 = ((2u * (v % 4) + 0u) ^ sw) << 4, c1 = ((2u * (v % 4) + 1u) ^ sw) << 4;
             constexpr uint32_t HI = 8 * 1024;  // B rows 64..127: the high-nibble plane
             st_shared_v4(atom + c0, lo[0], lo[1], lo[2], lo[3]);
@@ -279,23 +193,12 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
           for (int a = 0; a < 2; ++a)
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
-              st_shared_v4(bt + a * Cfg::B_ATOM + off_r + (c << 4), 0u, 0u, 0u, 0u);
-              st_shared_v4(bt + a * Cfg::B_ATOM + off_r + 8 * 1024 + (c << 4), 0u, 0u, 0u, 0u);
+              st_shared_v4(sg.bt + a * Cfg::B_ATOM + off_r + (c << 4), 0u, 0u, 0u, 0u);
+              st_shared_v4(sg.bt + a * Cfg::B_ATOM + off_r + 8 * 1024 + (c << 4), 0u, 0u, 0u, 0u);
             }
         }
-        publish();
-      };
-      Pre pa, pb;
-      pa.ok = pb.ok = false;
-      load_pre(pa);
-      for (int it = grp; it < total_it; it += 2 * NSTAGES) {
-        load_pre(pb);
-        process(pa);
-        if (it + NSTAGES < total_it) {
-          load_pre(pa);
-          process(pb);
-        }
-      }
+        sg.publish();
+      });
     } else {
       // ---------------- 8-bit weights: thread r converts reduction row n = kb * 64 + r, rnd(scale[n] * W[n, k])
       struct PreB {
@@ -303,10 +206,9 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
         uint32_t s2;
       };
       const WT* scale = static_cast<const WT*>(p.wscale);
-      auto load_pre = [&](PreB& pr) {
-        if (f_it >= total_it) return;
-        const int n = f_kb * 64 + r;
-        const int k0 = (f_tile / p.num_m_blocks) * 128;
+      auto load_pre = [&](PreB& pr, const StageSeq<L::NSTAGES>& seq) {
+        const int n = seq.kb * 64 + r;
+        const int k0 = (seq.tile / p.num_m_blocks) * 128;
         const bool ok = n < p.N;
         const uint8_t* src = p.w + static_cast<size_t>(ok ? n : 0) * p.K + k0;
 #pragma unroll
@@ -315,10 +217,9 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
         // rows past N: zero bytes times a zero scale -> exact zeros (their gO columns are zero-filled as well)
         const WT sv = ok ? scale[n] : from_float<WT>(0.f);
         pr.s2 = static_cast<uint32_t>(*reinterpret_cast<const uint16_t*>(&sv)) * 0x00010001u;
-        advance();
       };
-      auto process = [&](const PreB& cur) {
-        mbar_wait_u32(empty_addr, phase ^ 1u);
+      sg.template run_ping_pong<PreB>(load_pre, [&](const PreB& cur) {
+        sg.wait_empty();
 #pragma unroll
         for (int v = 0; v < 8; ++v) {
           uint32_t o[8];
@@ -326,22 +227,12 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
           cvt_bytes4<WT, Cfg::WKIND>(cur.raw[v].y, cur.s2, o[2], o[3]);
           cvt_bytes4<WT, Cfg::WKIND>(cur.raw[v].z, cur.s2, o[4], o[5]);
           cvt_bytes4<WT, Cfg::WKIND>(cur.raw[v].w, cur.s2, o[6], o[7]);
-          const uint32_t atom = bt + (v / 4) * Cfg::B_ATOM + off_r;
+          const uint32_t atom = sg.bt + (v / 4) * Cfg::B_ATOM + off_r;
           st_shared_v4(atom + (((2u * (v % 4) + 0u) ^ sw) << 4), o[0], o[1], o[2], o[3]);
           st_shared_v4(atom + (((2u * (v % 4) + 1u) ^ sw) << 4), o[4], o[5], o[6], o[7]);
         }
-        publish();
-      };
-      PreB pa, pb;
-      load_pre(pa);
-      for (int it = grp; it < total_it; it += 2 * NSTAGES) {
-        load_pre(pb);
-        process(pa);
-        if (it + NSTAGES < total_it) {
-          load_pre(pa);
-          process(pb);
-        }
-      }
+        sg.publish();
+      });
     }
   }
 }

@@ -1,6 +1,6 @@
 // Host-side plumbing shared by the translation units that hold the extern "C" entry points: status reporting,
-// per-DEVICE caches (SM count, architecture check, dynamic shared-memory opt-in), TMA descriptor encoding and the
-// test hooks that pick among equivalent kernels.
+// per-DEVICE caches (SM count, architecture check, dynamic shared-memory opt-in), the persistent-kernel launch, TMA
+// descriptor encoding and the test hooks that pick among equivalent kernels.
 #pragma once
 
 #include <atomic>
@@ -58,6 +58,17 @@ cudaError_t launch_kernel_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
+// Launch a persistent wgmma kernel (wgmma_pipe.cuh): one CTA per SM, or per tile when there are fewer tiles.  Layout is
+// the kernel's PipeLayout, which fixes its block size and dynamic shared memory.
+template <auto kernel, class Layout, class... Args>
+int launch_persistent(int tiles, cudaStream_t stream, const char* what, const Args&... args) {
+  int rc = ensure_dyn_smem<kernel>(Layout::SMEM_BYTES);
+  if (rc != OK) return rc;
+  const int grid = tiles < current_sm_count() ? tiles : current_sm_count();
+  kernel<<<grid, Layout::NTHREADS, Layout::SMEM_BYTES, stream>>>(args...);
+  return check_cuda(cudaGetLastError(), what);
+}
+
 // Row-major [rows, cols] matrix of `dt` elements; box = 128 bytes of a row x box_rows rows, 128-byte swizzle.
 int make_tmap_2d(CUtensorMap* map, const void* base, int dt, int64_t rows, int64_t cols, int box_rows);
 // Row-major [rows, cols] 16-bit matrix described as [rows, 2, cols/2] (two column planes); box = 64 elements of one
@@ -78,6 +89,22 @@ enum : int { ROUTE_AUTO = 0, ROUTE_INT4_GENERAL = 1, ROUTE_INT4_GEMV = 3, ROUTE_
 // OVR_QBYTES_ROUTE values
 enum : int { ROUTE_QBYTES_SIMT = 2 };
 int test_override(int key);
+
+// Rows per wgmma tile: one consumer warpgroup (64 rows) while M <= 64, so that small batches do not pay for empty MMA
+// rows, else 128; test override OVR_TILE_M forces either.
+inline int wgmma_tile_m(int64_t m) {
+  int tile_m = m <= 64 ? 64 : 128;
+  const int force_m = test_override(OVR_TILE_M);
+  if (force_m == 64 || force_m == 128) tile_m = force_m;
+  return tile_m;
+}
+
+// log2(group) when group is a power of two, else -1
+inline int group_log2(int group) {
+  for (int b = 0; b < 31; ++b)
+    if ((1 << b) == group) return b;
+  return -1;
+}
 
 // ---- developer knock-outs: only a KNOCKOUTS=1 build honours them; a release build reports and uses 0
 int debug_flags();
