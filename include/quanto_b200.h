@@ -216,6 +216,28 @@ QB200_API int qb200_absmax(const void* base, void* out, void* scratch, int64_t n
 QB200_API int qb200_quantize_qbytes_absmax(const void* base, void* out, void* scale, int64_t n, int64_t k, int dtype,
                                            int out_dtype, void* stream);
 
+/* freeze() of an axis-0 int4/int2 weight with the HQQ optimizer in TWO launches and no host synchronisation:
+ * HqqOptimizer (optimum/quanto/tensor/optimizers/hqq_optimizer.py:28-34 shrink_lp_op, :60-87 optimize, after
+ * max_optimizer.py:26-37) + affine_optimizer.py:52-63 (zeropoint) + quanto::quantize_affine + pack_weights.
+ * Outputs as qb200_quantize_qbits_max.  `errors`: float32 [iters + 2], the dt-rounded tensor-wide mean errors of the
+ * all-accepted trajectory (start error, then one per iteration), then the number of accepted iterations.
+ * `workspace`: qb200_quantize_qbits_hqq_workspace_bytes(n, k, group, iters) bytes of device memory, 256-byte aligned,
+ * owned by the call until the stream reaches its end.  bf16 / fp16 only, group % 8 == 0, group <= 256, iters <= 64,
+ * lp_norm > 0 (not 4, where torch's pow is a cube); else QB200_ERR_UNSUPPORTED.  Bit-exact with the reference's CPU
+ * arithmetic for the scale, shift and packed codes; the stop index follows from the dt-rounded means. */
+QB200_API int qb200_quantize_qbits_hqq(const void* base, uint8_t* packed, void* scale, void* shift, float* errors,
+                                       void* workspace, int64_t n, int64_t k, int group, int bits, int dtype,
+                                       int zeropoint, double lp_norm, double beta, double kappa, int iters, void* stream);
+
+/* Bytes of workspace qb200_quantize_qbits_hqq needs (0 for an invalid shape). */
+QB200_API int64_t qb200_quantize_qbits_hqq_workspace_bytes(int64_t n, int64_t k, int group, int iters);
+
+/* shrink_lp_op(x, beta, lp_norm) (optimum/quanto/tensor/optimizers/hqq_optimizer.py:28-34) elementwise on `numel`
+ * bf16 / fp16 values: the device shrink qb200_quantize_qbits_hqq uses, exposed so that it can be checked on every input.
+ * Same configurations as qb200_quantize_qbits_hqq. */
+QB200_API int qb200_hqq_shrink(const void* x, void* out, int64_t numel, double beta, double lp_norm, int dtype,
+                               void* stream);
+
 /* Which kernel family the last qb200_qbytes_mm / qb200_qbits_mm / *_grad_input call on this thread dispatched to:
  * 0 none, 1 wgmma (TMA + warpgroup MMA), 2 CUDA-core (shape-agnostic), 3 warp-MMA gemv (int4, M <= 32: TMA ring or register streaming).
  * For tests and bench accounting. */

@@ -55,6 +55,9 @@ EXPORTS = (
     "qb200_qbits_ring_plan",
     "qb200_qbits_mm_grad_input",
     "qb200_qbytes_mm_grad_input",
+    "qb200_quantize_qbits_hqq",
+    "qb200_quantize_qbits_hqq_workspace_bytes",
+    "qb200_hqq_shrink",
 )
 
 # qb200_test_override keys (include/quanto_b200.h)
@@ -134,6 +137,12 @@ def load():
         lib.qb200_quantize_qbytes_absmax.argtypes = [vp, vp, vp, i64, i64, i32, i32, vp]
         lib.qb200_qbits_mm_grad_input.argtypes = [vp, vp, vp, vp, vp, i64, i64, i64, i32, i32, i32, vp]
         lib.qb200_qbytes_mm_grad_input.argtypes = [vp, vp, vp, vp, i64, i64, i64, i32, i32, vp]
+        f64 = ctypes.c_double
+        lib.qb200_quantize_qbits_hqq.argtypes = [vp, vp, vp, vp, vp, vp, i64, i64, i32, i32, i32, i32, f64, f64, f64,
+                                                 i32, vp]
+        lib.qb200_quantize_qbits_hqq_workspace_bytes.argtypes = [i64, i64, i32, i32]
+        lib.qb200_quantize_qbits_hqq_workspace_bytes.restype = i64
+        lib.qb200_hqq_shrink.argtypes = [vp, vp, i64, f64, f64, i32, vp]
         for name in EXPORTS:
             getattr(lib, name)  # AttributeError here == header and library out of sync
         # Developer knock-outs exist only in a `make KNOCKOUTS=1` build and are set explicitly through

@@ -21,7 +21,10 @@ After this, every `optimum.quanto` object keeps working as before -- `quantize()
    `torch.matmul(gO, other)` on a dequantised dense copy) and keeps the reference's weight and bias gradients;
 4. `WeightQBytesLinearFunction.forward` (tensor/weights/qbytes.py:68-82) keeps calling `quanto::qbytes_mm`, with the bias
    fused into the kernel epilogue when there is one; its backward takes the input gradient from
-   `quanto::qbytes_grad_input` the same way.
+   `quanto::qbytes_grad_input` the same way;
+5. `HqqOptimizer.__call__` (tensor/optimizers/hqq_optimizer.py:60-87 after affine_optimizer.py:27-64) runs
+   `quanto::quantize_qbits_hqq` -- two launches, no host synchronisation -- for a CUDA bf16 / fp16 weight quantized along
+   axis 0 to qint4 / qint2, and the reference's own code for everything else and whatever the kernel declines.
 
 Used by tools/run_reference_tests.py to run the reference's OWN hot-path tests (tests/library, tests/tensor/ops,
 tests/nn/test_qlinear.py) against these kernels.  Nothing here is imported by the rest of the package.
@@ -132,4 +135,23 @@ def bind_reference():
             return linear_backward(ctx, gO, qbytes_grad_input)
 
     ref_qbytes.WeightQBytesLinearFunction = FusedQBytesLinear
+
+    # ---- 5. HQQ shift search on the device
+    from optimum.quanto.tensor.optimizers import HqqOptimizer as RefHqq
+
+    from .tensor.optimizers import HqqOptimizer
+    from .tensor.qtype import qint2, qint4
+
+    orig_hqq_call = RefHqq.__call__
+
+    def hqq_call(self, base, qtype, axis, group_size=None, zeropoint=False):
+        qt = {2: qint2, 4: qint4}.get(qtype.bits) if qtype.name in ("qint2", "qint4") else None
+        if qt is not None:
+            opt = HqqOptimizer(self.lp_norm, self.beta, self.kappa, self.iters, self.verbose)
+            fused = opt.fused(base, qt, axis, group_size, zeropoint)
+            if fused is not None:
+                return fused[1], fused[2]
+        return orig_hqq_call(self, base, qtype, axis, group_size, zeropoint)
+
+    RefHqq.__call__ = hqq_call
     _bound = True

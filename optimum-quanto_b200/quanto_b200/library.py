@@ -18,6 +18,8 @@ and the weight-freeze / calibration ops of the step before the path (SURVEY.md 8
   quanto::pack                    pack_weights (optimum/quanto/tensor/packed.py:24-69) as one launch
   quanto::quantize_qbits_max      MaxOptimizer + quantize_affine + pack_weights in one launch (axis 0)
   quanto::quantize_qbytes_absmax  AbsmaxOptimizer + quantize_symmetric in one launch (axis 0)
+  quanto::quantize_qbits_hqq      HqqOptimizer + quantize_affine + pack_weights in two launches (axis 0)
+  quanto::hqq_shrink              shrink_lp_op of HqqOptimizer (optimum/quanto/tensor/optimizers/hqq_optimizer.py:28-34)
   quanto::absmax                  per-tensor max|x| (optimum/quanto/calibrate.py:37-61)
 
 Only the CUDA dispatch key gets a kernel.  There is deliberately no CPU implementation of the hot-path ops: calling
@@ -67,6 +69,9 @@ _define("pack", "(Tensor self, int bits) -> Tensor")
 _define("quantize_qbits_max", "(Tensor base, int bits, int group_size, bool zeropoint) -> (Tensor, Tensor, Tensor)")
 _define("quantize_qbytes_absmax", "(Tensor base, ScalarType dtype) -> (Tensor, Tensor)")
 _define("absmax", "(Tensor base) -> Tensor")
+_define("quantize_qbits_hqq", "(Tensor base, int bits, int group_size, bool zeropoint, float lp_norm, float beta, "
+                              "float kappa, int iters) -> (Tensor, Tensor, Tensor, Tensor)")
+_define("hqq_shrink", "(Tensor x, float beta, float lp_norm) -> Tensor")
 _define("qbits_grad_input", "(Tensor grad_output, Tensor packed, Tensor scale, Tensor shift, int out_features, "
                             "int group_size, int bits) -> Tensor")
 _define("qbytes_grad_input", "(Tensor grad_output, Tensor B, Tensor scales) -> Tensor")
@@ -260,6 +265,57 @@ def quantize_qbits_max_cuda(base: torch.Tensor, bits: int, group_size: int, zero
                                              bits, N.DTYPE_CODE[base.dtype], 1 if zeropoint else 0,
                                              N.stream_ptr(base.device)), "quanto::quantize_qbits_max")
     return packed, scale, shift
+
+
+def quantize_qbits_hqq_cuda(base: torch.Tensor, bits: int, group_size: int, zeropoint: bool, lp_norm: float,
+                            beta: float, kappa: float, iters: int):
+    """HqqOptimizer + quantize_affine + pack_weights for an axis-0 weight [N, K] in two launches, no host sync.
+
+    Returns (packed, scale, shift) as quanto::quantize_qbits_max does, for the scale and shift that
+    `HqqOptimizer(lp_norm, beta, kappa, iters)(base, qtype, axis=0, group_size, zeropoint)` returns
+    (optimum/quanto/tensor/optimizers/hqq_optimizer.py:60-87), and `errors` (float32 [iters + 2]): the dt-rounded mean
+    errors of the all-accepted trajectory (start error, then one per iteration), then the accepted count.  Raises
+    UnsupportedConfiguration for what the kernel does not take (float32, group > 256, iters > 64, ...).
+    """
+    if base.ndim != 2:
+        raise ValueError("quantize_qbits_hqq expects a 2-D weight [out_features, in_features]")
+    if base.dtype not in _FLOATS:
+        raise ValueError(f"quantize_qbits_hqq: unsupported dtype {base.dtype}")
+    if bits not in (2, 4):
+        raise ValueError("bits must be 2 or 4")
+    n, k = base.shape
+    if group_size <= 0 or k % group_size != 0:
+        raise ValueError(f"Group size ({group_size}) must be a divisor of ({k})")
+    base = _require_contiguous(base, "base")
+    rows = n * k // group_size
+    per_byte = 8 // bits
+    packed = torch.empty((-(-rows // per_byte), group_size), dtype=torch.uint8, device=base.device)
+    scale = torch.empty((rows, 1), dtype=base.dtype, device=base.device)
+    shift = torch.empty((rows, 1), dtype=torch.uint8 if zeropoint else base.dtype, device=base.device)
+    errors = torch.empty(max(iters, 0) + 2, dtype=torch.float32, device=base.device)
+    with torch.cuda.device(base.device):
+        lib = N.load()
+        ws_bytes = lib.qb200_quantize_qbits_hqq_workspace_bytes(n, k, group_size, iters)
+        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=base.device)
+        N.check(lib.qb200_quantize_qbits_hqq(N.ptr(base), N.ptr(packed), N.ptr(scale), N.ptr(shift), N.ptr(errors),
+                                             N.ptr(ws), n, k, group_size, bits, N.DTYPE_CODE[base.dtype],
+                                             1 if zeropoint else 0, lp_norm, beta, kappa, iters,
+                                             N.stream_ptr(base.device)), "quanto::quantize_qbits_hqq")
+    return packed, scale, shift, errors
+
+
+def hqq_shrink_cuda(x: torch.Tensor, beta: float, lp_norm: float) -> torch.Tensor:
+    """shrink_lp_op(x, beta, lp_norm) (optimum/quanto/tensor/optimizers/hqq_optimizer.py:28-34) with the device
+    arithmetic quanto::quantize_qbits_hqq uses; bf16 / fp16."""
+    if x.dtype not in _FLOATS:
+        raise ValueError(f"hqq_shrink: unsupported dtype {x.dtype}")
+    x = _require_contiguous(x, "x")
+    out = torch.empty_like(x)
+    with torch.cuda.device(x.device):
+        lib = N.load()
+        N.check(lib.qb200_hqq_shrink(N.ptr(x), N.ptr(out), x.numel(), beta, lp_norm, N.DTYPE_CODE[x.dtype],
+                                     N.stream_ptr(x.device)), "quanto::hqq_shrink")
+    return out
 
 
 def quantize_qbytes_absmax_cuda(base: torch.Tensor, dtype: torch.dtype):
@@ -551,6 +607,8 @@ _bind_cuda("pack", pack_cuda)
 _bind_cuda("quantize_qbits_max", quantize_qbits_max_cuda)
 _bind_cuda("quantize_qbytes_absmax", quantize_qbytes_absmax_cuda)
 _bind_cuda("absmax", absmax_cuda)
+_bind_cuda("quantize_qbits_hqq", quantize_qbits_hqq_cuda)
+_bind_cuda("hqq_shrink", hqq_shrink_cuda)
 _bind_cuda("quantize_affine", quantize_affine_cuda)
 try:
     _lib.impl("quantize_affine", quantize_affine_any, "CompositeExplicitAutograd")

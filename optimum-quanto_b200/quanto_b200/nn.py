@@ -10,9 +10,9 @@ from typing import Optional, Union
 import torch
 
 from . import _native
-from .tensor import (AbsmaxOptimizer, ActivationQBytesTensor, MaxOptimizer, Optimizer, QTensor, SymmetricOptimizer,
-                     PackedTensor, WeightQBitsTensor, WeightQBytesTensor, qint2, qint4, qtype, qtypes, quantize_activation,
-                     quantize_weight)
+from .tensor import (AbsmaxOptimizer, ActivationQBytesTensor, HqqOptimizer, MaxOptimizer, Optimizer, QTensor,
+                     SymmetricOptimizer, PackedTensor, WeightQBitsTensor, WeightQBytesTensor, qint2, qint4, qtype, qtypes,
+                     quantize_activation, quantize_weight)
 
 __all__ = ["QModuleMixin", "QLinear", "freeze"]
 
@@ -157,6 +157,15 @@ class QModuleMixin:
                 packed, scale, shift = torch.ops.quanto.quantize_qbits_max(w.detach(), qt.bits, group, False)
             except _native.UnsupportedConfiguration:
                 return None
+            rows = w.numel() // group
+            data = PackedTensor(packed, qt.bits, torch.Size([rows, group]), (group, 1))
+            return WeightQBitsTensor(qt, 0, self.weight_group_size, w.size(), w.stride(), data, scale, shift)
+        if qt in (qint2, qint4) and type(self.optimizer) is HqqOptimizer:
+            group = self.weight_group_size or w.shape[1]
+            fused = self.optimizer.fused(w.detach(), qt, 0, group)
+            if fused is None:
+                return None
+            packed, scale, shift = fused
             rows = w.numel() // group
             data = PackedTensor(packed, qt.bits, torch.Size([rows, group]), (group, 1))
             return WeightQBitsTensor(qt, 0, self.weight_group_size, w.size(), w.stride(), data, scale, shift)
