@@ -252,7 +252,9 @@ QB200_API int qb200_last_kernel_family(void);
  *   key 3  qbytes route                    : 2 CUDA-core kernel
  *   key 4  ring-gemv producer              : 1 one issuing thread, 2 one lane per packed row, 3 32 lanes
  *   key 5  programmatic dependent launch   : 1 off
- *   key 6  ring-gemv shape (M <= 2)        : 2 two CTAs per SM (opt-in experiment; default one CTA per SM) */
+ *   key 6  ring-gemv shape (M <= 2)        : 2 two CTAs per SM (opt-in experiment; default one CTA per SM)
+ *   key 7  int4 wgmma epilogue             : 1 ordinary stores (default: TMA stores from a shared-memory tile when the
+ *                                            output is one dense [M, N] buffer with N % 16 == 0) */
 QB200_API int qb200_test_override(int key, int value);
 
 /* Developer aids.  They act only in a library built with `make KNOCKOUTS=1` (qb200_developer_build() == 1); in the

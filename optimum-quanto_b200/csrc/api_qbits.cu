@@ -13,22 +13,23 @@ int launch_qbits_mm_simt(const void*, const uint8_t*, const void*, const void*, 
                          int, int, int, int64_t, int64_t, cudaStream_t);
 
 template <class Cfg>
-static int launch_gemm(const CUtensorMap& ta, const GemmParams& p, cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tout, const GemmParams& p, cudaStream_t stream) {
   CUtensorMap tb;
   std::memset(&tb, 0, sizeof(tb));  // the weight tile is staged by the kernel's own warps
   return launch_persistent<gemm_tc_kernel<Cfg>, typename Cfg::Pipe>(p.num_m_blocks * p.num_n_blocks, stream,
-                                                                    "gemm_tc_kernel launch", ta, tb, p);
+                                                                    "gemm_tc_kernel launch", ta, tb, tout, p);
 }
 
 template <int MWG>
-static int launch_int4(const CUtensorMap& ta, const GemmParams& p, int dtype, bool zp, cudaStream_t st) {
+static int launch_int4(const CUtensorMap& ta, const CUtensorMap& tout, const GemmParams& p, int dtype, bool zp,
+                       cudaStream_t st) {
   constexpr int BN = 128;
   if (dtype == DT_BF16) {
-    if (zp) return launch_gemm<GemmCfg<MmaKind::BF16, BSrc::INT4, MWG, BN, __nv_bfloat16, true>>(ta, p, st);
-    return launch_gemm<GemmCfg<MmaKind::BF16, BSrc::INT4, MWG, BN, __nv_bfloat16, false>>(ta, p, st);
+    if (zp) return launch_gemm<GemmCfg<MmaKind::BF16, BSrc::INT4, MWG, BN, __nv_bfloat16, true>>(ta, tout, p, st);
+    return launch_gemm<GemmCfg<MmaKind::BF16, BSrc::INT4, MWG, BN, __nv_bfloat16, false>>(ta, tout, p, st);
   }
-  if (zp) return launch_gemm<GemmCfg<MmaKind::F16, BSrc::INT4, MWG, BN, __half, true>>(ta, p, st);
-  return launch_gemm<GemmCfg<MmaKind::F16, BSrc::INT4, MWG, BN, __half, false>>(ta, p, st);
+  if (zp) return launch_gemm<GemmCfg<MmaKind::F16, BSrc::INT4, MWG, BN, __half, true>>(ta, tout, p, st);
+  return launch_gemm<GemmCfg<MmaKind::F16, BSrc::INT4, MWG, BN, __half, false>>(ta, tout, p, st);
 }
 
 static int qbits_mm_impl(QbitsArgs& q) {
@@ -86,10 +87,21 @@ static int qbits_mm_impl(QbitsArgs& q) {
   CUtensorMap ta;
   rc = make_tmap_2d(&ta, q.a, dtype, m, k, tile_m);
   if (rc != OK) return rc;
+  // The epilogue stores each warpgroup's 64 x 128 tile with TMA when the output is one dense, 16-byte aligned [M, N]
+  // buffer whose two nibble planes [M, 2, N/2] have 16-byte aligned rows (N % 16 == 0).  Everything else -- the fused
+  // gather's peer buffers and column slab, N % 16 != 0, a map the driver declines -- stores with ordinary stores.
+  CUtensorMap tout;
+  std::memset(&tout, 0, sizeof(tout));
+  p.epi_tma = 0;
+  if (test_override(OVR_INT4_EPILOGUE) != 1 && q.g.n_out == 1 && q.g.out_peer[0] == q.out && q.ld == n && q.col0 == 0 &&
+      n % 16 == 0 && reinterpret_cast<uintptr_t>(q.out) % 16 == 0) {
+    if (make_tmap_planes(&tout, q.out, dtype, m, n, 64) == OK) p.epi_tma = 1;
+    else std::memset(&tout, 0, sizeof(tout));
+  }
   set_kernel_family(1);
   const bool zp = q.shift_is_int != 0;
-  if (tile_m == 64) return launch_int4<1>(ta, p, dtype, zp, q.stream);
-  return launch_int4<2>(ta, p, dtype, zp, q.stream);
+  if (tile_m == 64) return launch_int4<1>(ta, tout, p, dtype, zp, q.stream);
+  return launch_int4<2>(ta, tout, p, dtype, zp, q.stream);
 }
 
 }  // namespace qb

@@ -15,8 +15,10 @@ int launch_qbytes_mm_simt(const void*, const void*, const void*, const void*, vo
 
 template <class Cfg>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream) {
+  CUtensorMap tout;
+  std::memset(&tout, 0, sizeof(tout));  // the 8-bit epilogues store straight from the accumulators
   return launch_persistent<gemm_tc_kernel<Cfg>, typename Cfg::Pipe>(p.num_m_blocks * p.num_n_blocks, stream,
-                                                                    "gemm_tc_kernel launch", ta, tb, p);
+                                                                    "gemm_tc_kernel launch", ta, tb, tout, p);
 }
 
 // Columns of tensor-core work per SM for a tile of BM x bn: waves x bn (wave quantisation included).

@@ -110,6 +110,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) { mbar
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
 __device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
   uint4 v;
   asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
@@ -142,6 +150,21 @@ __device__ __forceinline__ void bulk_wait_group_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
 __device__ __forceinline__ void bulk_wait_group_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+// 3-D tiled TMA store of one box from shared memory (coordinates innermost first), tracked by the issuing thread's bulk
+// async-group: commit it with bulk_commit_group(), and bulk_wait_group_read before the source is written again.  TMA
+// writes only the part of the box inside the tensor map's dimensions.
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t smem_src, int32_t c0, int32_t c1,
+                                             int32_t c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+
+// Named barrier `id` (1..15; 0 is __syncthreads) over `nthreads` threads, a multiple of 32.
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 // ------------------------------------------------------------------------------------------------
 // wgmma (Hopper warpgroup MMA): D[64 x N] (+)= A[64 x K] * B[N x K]^T, both operands K-major in shared memory,

@@ -63,6 +63,9 @@ struct GemmParams {
   // cast exactly like quanto::quantize_symmetric; `out` is then a [M, ld] buffer of BYTES.
   int q_dt;
   const void* q_scale;
+  // BSrc::INT4: 1 = the epilogue stores each tile with TMA through `tmap_out` (one dense [M, N] output: g.n_out = 1,
+  // ld = N, col0 = 0, N % 16 == 0); 0 = ordinary stores
+  int epi_tma;
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -324,8 +327,11 @@ struct GemmCfg {
   // per one or two activation rows) per stage slot.  3 slots keep the CTA at 15 warps, which leaves 128 registers per thread (the consumers hold 64 accumulators).
   static constexpr int NSTAGES =
       (BSRC == BSrc::TMA) ? ((192 * 1024) / (A_TILE + B_TILE) > 8 ? 8 : (192 * 1024) / (A_TILE + B_TILE)) : 3;
+  // int4: one 64 x BN output staging tile of the activation dtype per consumer warpgroup (int4_epilogue)
+  static constexpr int EPI_TILE = (BSRC == BSrc::INT4) ? 64 * BN * 2 : 0;
   // the TMA producer's arrive (A tile, and W for TMA) + one per staging warp; F8 stages both operands without TMA
-  using Pipe = PipeLayout<MWG, NSTAGES, A_TILE, B_TILE, (BSRC == BSrc::TMA) ? 0 : BN / 64, (BSRC == BSrc::F8) ? 0 : 1>;
+  using Pipe = PipeLayout<MWG, NSTAGES, A_TILE, B_TILE, (BSRC == BSrc::TMA) ? 0 : BN / 64, (BSRC == BSrc::F8) ? 0 : 1,
+                          MWG * EPI_TILE>;
   static_assert(BN == 128 || (BN == 256 && IS_INT && BSRC == BSrc::TMA), "wgmma tile width");
   static_assert(BSRC == BSrc::TMA || KIND == MmaKind::F16 || KIND == MmaKind::BF16, "staged weights are 16-bit");
 };
@@ -401,19 +407,104 @@ __device__ __forceinline__ void epilogue_pair(const GemmParams& p, size_t row_of
   else epilogue_pair_t<float, ALLOW_Q>(p, row_off, n, two, f0, f1);
 }
 
+// Epilogue of the int4 kernels (output dtype OT = the 16-bit activation dtype), one consumer warpgroup's 64-row slice
+// of a 64 x 128 tile.  The tile's columns [0, 64) are the low-nibble out-features n_blk * 64 + c, its columns
+// [64, 128) the high-nibble ones N/2 + n_blk * 64 + c - 64.
+//   1. The warpgroup rounds its accumulators, rnd_OT(acc) (+ bias, rounded), into its staging tile `stile`: two planes
+//      of 64 rows x 64 columns (low- and high-nibble columns), each row 128 bytes with the 128-byte swizzle.
+//   2. p.epi_tma: one thread stores the two planes with TMA into the output seen as [M, 2, N/2] (`tmap_out`, box 64
+//      columns x 1 plane x 64 rows); TMA drops what lies past M or past the end of a plane.  The store completes while
+//      the next tile's mainloop runs; the next epilogue waits until it has read the staging tile.
+//      Otherwise the warpgroup copies the tile out with ordinary, bounds-checked stores into every output buffer of
+//      the fused gather, at the row pitch `ld` and column offset `col0`.
+constexpr int kInt4EpiPlane = 64 * 128;  // bytes of one staging plane
+template <typename OT>
+__device__ __forceinline__ void int4_epilogue(const GemmParams& p, const CUtensorMap* tmap_out, const float (&acc)[64],
+                                              uint32_t stile, int row0, int n_blk, int wg) {
+  const int t = threadIdx.x & 127;
+  const int lane = t & 31;
+  const int half_n = p.N / 2;
+  const OT* bias = static_cast<const OT*>(p.bias);
+  // the staging tile is free: the previous tile's TMA store has read it, and every thread has finished copying it out
+  if (t == 0) bulk_wait_group_read<0>();
+  named_bar_sync(1 + wg, 128);
+  // fragment (common.cuh): acc[4 j + 2 h + e] is row 16 (t / 32) + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e.  Row r
+  // of a plane lives at r * 128 with 16-byte chunk c at c ^ (r % 8), and r % 8 == lane / 4: the 32 lanes of a warp
+  // write 32 different banks.
+  const uint32_t sw = static_cast<uint32_t>(lane) >> 2;
+  const uint32_t row_addr = stile + static_cast<uint32_t>((t >> 5) * 16 + (lane >> 2)) * 128 + (lane & 3) * 4;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int n = (j < 8 ? 0 : half_n) + n_blk * 64 + 8 * (j & 7) + 2 * (lane & 3);
+    const int n_limit = j < 8 ? half_n : p.N;
+    float b0 = 0.f, b1 = 0.f;
+    if (bias != nullptr) {
+      if (n < n_limit) b0 = to_float<OT>(bias[n]);
+      if (n + 1 < n_limit) b1 = to_float<OT>(bias[n + 1]);
+    }
+    const uint32_t a = row_addr + (j >> 3) * kInt4EpiPlane + ((static_cast<uint32_t>(j & 7) ^ sw) << 4);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+      rnd_pair<OT>(f0, f1);
+      if (bias != nullptr) {
+        f0 = __fadd_rn(f0, b0);
+        f1 = __fadd_rn(f1, b1);
+        rnd_pair<OT>(f0, f1);
+      }
+      st_shared_u32(a + h * 8 * 128, pack2<OT>(f0, f1));
+    }
+  }
+  fence_proxy_async_smem();  // the tile's generic-proxy writes -> visible to the TMA store
+  named_bar_sync(1 + wg, 128);
+  if (p.epi_tma) {
+    if (t == 0 && row0 < p.M) {
+      tma_store_3d(tmap_out, stile, n_blk * 64, 0, row0);
+      tma_store_3d(tmap_out, stile + kInt4EpiPlane, n_blk * 64, 1, row0);
+      bulk_commit_group();
+    }
+    return;
+  }
+  // copy-out: thread t moves column pair 2 (t % 64) of rows t / 64, t / 64 + 2, ...: a warp reads one 128-byte plane row
+  // and writes 32 consecutive pairs
+  const int c = 2 * (t & 63);
+  const int plane = c >> 6, pc = c & 63;
+  const int n = (plane ? half_n : 0) + n_blk * 64 + pc;
+  const int n_limit = plane ? p.N : half_n;
+  if (n >= n_limit) return;
+  const bool two = n + 1 < n_limit;
+  const uint32_t src = stile + plane * kInt4EpiPlane + (pc & 7) * 2;
+  for (int r = t >> 6; r < 64 && row0 + r < p.M; r += 2) {
+    const uint32_t v = ld_shared_u32(src + r * 128 + ((static_cast<uint32_t>(pc >> 3) ^ (r & 7)) << 4));
+    const size_t off = static_cast<size_t>(row0 + r) * p.ld + p.col0 + n;
+    const bool vec = (off * sizeof(OT)) % (2 * sizeof(OT)) == 0;
+    for (int q = 0; q < p.g.n_out; ++q) {
+      uint16_t* dst = static_cast<uint16_t*>(p.g.out_peer[q]) + off;
+      if (two && vec) {
+        *reinterpret_cast<uint32_t*>(dst) = v;
+      } else {
+        dst[0] = static_cast<uint16_t>(v);
+        if (two) dst[1] = static_cast<uint16_t>(v >> 16);
+      }
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // The kernel
 // ------------------------------------------------------------------------------------------------
 template <class Cfg>
 __global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
     gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                   const GemmParams p) {
+                   const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
   using L = typename Cfg::Pipe;
   constexpr int BN = Cfg::BN;
 
   const auto pipe = WgmmaPipe<L>::init([&] {
     tma_prefetch_desc(&tmap_a);
     if constexpr (Cfg::BSRC == BSrc::TMA) tma_prefetch_desc(&tmap_b);
+    if constexpr (Cfg::BSRC == BSrc::INT4)
+      if (p.epi_tma) tma_prefetch_desc(&tmap_out);
   });
 
   const int warp = threadIdx.x >> 5;
@@ -430,49 +521,42 @@ __global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
     using AccT = typename std::conditional<Cfg::IS_INT, uint32_t, float>::type;
     AccT acc[Cfg::NACC];
     RingPos<L::NSTAGES> pos;
-    const int half_n = p.N / 2;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m_blk = tile % p.num_m_blocks;
       const int n_blk = tile / p.num_m_blocks;
       pipe.consume_tile(pos, kblocks, acc, [&](uint32_t aa, uint32_t bb, bool accumulate) {
         wgmma_slab<Cfg::KIND, BN>(acc, aa, bb, accumulate);
       });
-      // epilogue straight from the fragment: thread holds rows r0 and r0 + 8, column pairs 8 j + 2 (lane % 4)
-      const int r0 = m_blk * Cfg::BM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+      if constexpr (Cfg::BSRC == BSrc::INT4) {
+        int4_epilogue<typename Cfg::WT>(p, &tmap_out, acc, pipe.epi + wg * Cfg::EPI_TILE, m_blk * Cfg::BM + wg * 64,
+                                        n_blk, wg);
+      } else {
+        // epilogue straight from the fragment: thread holds rows r0 and r0 + 8, column pairs 8 j + 2 (lane % 4)
+        const int r0 = m_blk * Cfg::BM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = r0 + 8 * h;
-        if (row >= p.M) continue;
-        const size_t row_off = static_cast<size_t>(row) * p.ld + p.col0;
+        for (int h = 0; h < 2; ++h) {
+          const int row = r0 + 8 * h;
+          if (row >= p.M) continue;
+          const size_t row_off = static_cast<size_t>(row) * p.ld + p.col0;
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int c = 8 * j + 2 * (lane & 3);
-          // tile column -> output feature.  int4: columns [0, BN/2) are the low-nibble rows, [BN/2, BN) the high-nibble
-          // rows (+N/2)
-          int n, n_limit;
-          if constexpr (Cfg::BSRC == BSrc::INT4) {
-            if (c < BN / 2) { n = n_blk * (BN / 2) + c; n_limit = half_n; }
-            else { n = half_n + n_blk * (BN / 2) + (c - BN / 2); n_limit = p.N; }
-          } else {
-            n = n_blk * BN + c;
-            n_limit = p.N;
+          for (int j = 0; j < BN / 8; ++j) {
+            const int n = n_blk * BN + 8 * j + 2 * (lane & 3);
+            if (n >= p.N) continue;
+            float f0, f1;
+            if constexpr (Cfg::IS_INT) {
+              f0 = __int2float_rn(static_cast<int>(acc[4 * j + 2 * h]));
+              f1 = __int2float_rn(static_cast<int>(acc[4 * j + 2 * h + 1]));
+            } else {
+              f0 = acc[4 * j + 2 * h];
+              f1 = acc[4 * j + 2 * h + 1];
+            }
+            epilogue_pair<Cfg::BSRC == BSrc::TMA || Cfg::BSRC == BSrc::F8>(p, row_off, n, n + 1 < p.N, f0, f1);
           }
-          if (n >= n_limit) continue;
-          float f0, f1;
-          if constexpr (Cfg::IS_INT) {
-            f0 = __int2float_rn(static_cast<int>(acc[4 * j + 2 * h]));
-            f1 = __int2float_rn(static_cast<int>(acc[4 * j + 2 * h + 1]));
-          } else {
-            f0 = acc[4 * j + 2 * h];
-            f1 = acc[4 * j + 2 * h + 1];
-          }
-          // int4: the output dtype is the activation dtype, so the unrolled epilogue inlines one store path per pair
-          // instead of a runtime switch over three (the int4 GEMM at M = 4096 is epilogue-bound, DESIGN section 6)
-          if constexpr (Cfg::BSRC == BSrc::INT4) epilogue_pair_t<typename Cfg::WT, false>(p, row_off, n, n + 1 < n_limit, f0, f1);
-          else epilogue_pair<Cfg::BSRC == BSrc::TMA || Cfg::BSRC == BSrc::F8>(p, row_off, n, n + 1 < n_limit, f0, f1);
         }
       }
     }
+    if constexpr (Cfg::BSRC == BSrc::INT4)
+      if ((threadIdx.x & 127) == 0) bulk_wait_group_all();  // the last tile's TMA store has completed
     if (p.g.n_out > 1) __threadfence_system();  // this thread's peer stores are performed before the rank signals
   } else if (warp == L::PRODUCER_WARP) {
     // ------------------------------------------------------------------ TMA producer

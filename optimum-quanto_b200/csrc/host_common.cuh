@@ -83,7 +83,8 @@ int make_tmap_2d_view(CUtensorMap* map, const void* base, int dt, int64_t rows, 
 enum : int { OVR_TILE_M = 0 /* 64 | 128 rows per wgmma tile */, OVR_QBYTES_TILE_N = 1 /* int8: 128 | 256 */,
              OVR_INT4_ROUTE = 2, OVR_QBYTES_ROUTE = 3, OVR_GEMV_PRODUCER = 4,
              OVR_PDL = 5 /* 1 = no programmatic dependent launch */,
-             OVR_GEMV_SHAPE = 6 /* 2 = the two-CTAs-per-SM shape of the ring gemv (M <= 2) */, OVR_COUNT = 7 };
+             OVR_GEMV_SHAPE = 6 /* 2 = the two-CTAs-per-SM shape of the ring gemv (M <= 2) */,
+             OVR_INT4_EPILOGUE = 7 /* 1 = the int4 wgmma epilogue stores without TMA */, OVR_COUNT = 8 };
 // OVR_INT4_ROUTE values
 enum : int { ROUTE_AUTO = 0, ROUTE_INT4_GENERAL = 1, ROUTE_INT4_GEMV = 3, ROUTE_INT4_RING = 4, ROUTE_INT4_RING2 = 8 };
 // OVR_QBYTES_ROUTE values

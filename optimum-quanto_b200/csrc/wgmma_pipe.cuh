@@ -20,8 +20,9 @@
 namespace qb {
 
 // Warp roles and shared-memory budget from the kernel's tile choices.  TMA_ARRIVALS: arrivals of the TMA producer on
-// `full` per stage (0 when the staging warps write every operand); GROUP_WARPS: staging warps per stage slot.
-template <int MWG_, int NSTAGES_, int A_TILE_, int B_TILE_, int GROUP_WARPS_, int TMA_ARRIVALS_>
+// `full` per stage (0 when the staging warps write every operand); GROUP_WARPS: staging warps per stage slot;
+// EPI_BYTES: the consumers' output staging tiles, after the stages (a multiple of 1024 bytes, 0 when there are none).
+template <int MWG_, int NSTAGES_, int A_TILE_, int B_TILE_, int GROUP_WARPS_, int TMA_ARRIVALS_, int EPI_BYTES_ = 0>
 struct PipeLayout {
   static constexpr int MWG = MWG_;
   static constexpr int NSTAGES = NSTAGES_;
@@ -33,8 +34,10 @@ struct PipeLayout {
   static constexpr int FIRST_CVT_WARP = PRODUCER_WARP + 1;
   static constexpr int NTHREADS = (FIRST_CVT_WARP + NCVT_WARPS) * 32;
   static constexpr int FULL_ARRIVALS = TMA_ARRIVALS_ + CVT_GROUP_WARPS;
-  // 1024 bytes of alignment slack (the swizzled tiles need 1024-byte aligned bases) + the barriers
-  static constexpr int SMEM_BYTES = 1024 + NSTAGES * STAGE + 2 * NSTAGES * 8;
+  static constexpr int EPI_BYTES = EPI_BYTES_;
+  static_assert(EPI_BYTES % 1024 == 0, "output staging tiles keep the 1024-byte alignment of the swizzle");
+  // 1024 bytes of alignment slack (the swizzled tiles need 1024-byte aligned bases) + the output staging + the barriers
+  static constexpr int SMEM_BYTES = 1024 + NSTAGES * STAGE + EPI_BYTES + 2 * NSTAGES * 8;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
 };
 
@@ -66,6 +69,7 @@ struct WgmmaPipe {
   static constexpr int NSTAGES = L::NSTAGES;
   uint8_t* smem;       // stage 0; stage s at smem + s * STAGE, its A tile first, then its B tile
   uint32_t base;       // shared-memory address of stage 0
+  uint32_t epi;        // shared-memory address of the output staging tiles (EPI_BYTES, 1024-byte aligned)
   uint64_t* full_bar;  // [NSTAGES]: the stage's operands have landed
   uint64_t* empty_bar; // [NSTAGES]: every consumer warpgroup is done reading the stage
 
@@ -79,7 +83,8 @@ struct WgmmaPipe {
     WgmmaPipe pipe;
     pipe.smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
     pipe.base = smem_u32(pipe.smem);
-    pipe.full_bar = reinterpret_cast<uint64_t*>(pipe.smem + NSTAGES * L::STAGE);
+    pipe.epi = pipe.base + NSTAGES * L::STAGE;
+    pipe.full_bar = reinterpret_cast<uint64_t*>(pipe.smem + NSTAGES * L::STAGE + L::EPI_BYTES);
     pipe.empty_bar = pipe.full_bar + NSTAGES;
     if (threadIdx.x == L::PRODUCER_WARP * 32) {
       prefetch();

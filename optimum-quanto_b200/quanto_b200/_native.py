@@ -61,7 +61,8 @@ EXPORTS = (
 )
 
 # qb200_test_override keys (include/quanto_b200.h)
-OVR_TILE_M, OVR_QBYTES_TILE_N, OVR_INT4_ROUTE, OVR_QBYTES_ROUTE, OVR_GEMV_PRODUCER, OVR_PDL, OVR_GEMV_SHAPE = range(7)
+(OVR_TILE_M, OVR_QBYTES_TILE_N, OVR_INT4_ROUTE, OVR_QBYTES_ROUTE, OVR_GEMV_PRODUCER, OVR_PDL, OVR_GEMV_SHAPE,
+ OVR_INT4_EPILOGUE) = range(8)
 ROUTE_INT4_GENERAL, ROUTE_INT4_GEMV, ROUTE_INT4_RING, ROUTE_INT4_RING2 = 1, 3, 4, 8
 ROUTE_QBYTES_SIMT = 2
 GATHER_WAIT_INPUT, GATHER_WAIT_OUTPUT = 1, 2
