@@ -174,6 +174,10 @@ int make_tmap_planes(CUtensorMap* map, const void* base, int dt, int64_t rows, i
   return OK;
 }
 
+int make_tmap_packed(CUtensorMap* map, const uint8_t* packed, int64_t rows, int64_t cols, int box_rows) {
+  return encode_2d(map, packed, DT_U8, rows, cols, cols, 64, box_rows, CU_TENSOR_MAP_SWIZZLE_64B);
+}
+
 int make_tmap_2d_view(CUtensorMap* map, const void* base, int dt, int64_t rows, int64_t cols, int64_t pitch_elems,
                       int box_cols, int box_rows, bool swizzle128) {
   return encode_2d(map, base, dt, rows, cols, pitch_elems, box_cols, box_rows,

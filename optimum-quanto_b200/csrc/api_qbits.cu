@@ -32,6 +32,38 @@ static int launch_int4(const CUtensorMap& ta, const CUtensorMap& tout, const Gem
   return launch_gemm<GemmCfg<MmaKind::F16, BSrc::INT4, MWG, BN, __half, false>>(ta, tout, p, st);
 }
 
+template <int T>
+static int launch_w4(const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tout, const GemmParams& p,
+                     int dtype, bool zp, cudaStream_t st) {
+  const int tiles = p.num_m_blocks * p.num_n_blocks;
+  if (dtype == DT_BF16) {
+    if (zp) {
+      using C = W4Cfg<MmaKind::BF16, T, __nv_bfloat16, true>;
+      return launch_persistent<gemm_w4_kernel<C>, C>(tiles, st, "gemm_w4_kernel launch", ta, tw, tout, p);
+    }
+    using C = W4Cfg<MmaKind::BF16, T, __nv_bfloat16, false>;
+    return launch_persistent<gemm_w4_kernel<C>, C>(tiles, st, "gemm_w4_kernel launch", ta, tw, tout, p);
+  }
+  if (zp) {
+    using C = W4Cfg<MmaKind::F16, T, __half, true>;
+    return launch_persistent<gemm_w4_kernel<C>, C>(tiles, st, "gemm_w4_kernel launch", ta, tw, tout, p);
+  }
+  using C = W4Cfg<MmaKind::F16, T, __half, false>;
+  return launch_persistent<gemm_w4_kernel<C>, C>(tiles, st, "gemm_w4_kernel launch", ta, tw, tout, p);
+}
+
+// Which int4 wgmma kernel runs a problem of m_blocks token tiles and half_n packed rows.  The swap-AB kernel
+// (gemm_w4_kernel) does a tile of 128 packed rows in about 1.8x the time the weight-staging kernel (gemm_tc_kernel)
+// takes for its 64-row tile (H100 SXM, bf16, M = 4096: 1.10 vs 1.22 ms for twice the tiles), so it wins once its tiles
+// fill every SM and its waves, 1.8x as long, are fewer than 5/9 of the staging kernel's.  At N = 14336 on 132 SMs that
+// is M = 512, 768 and M >= 1536; small batches (M <= 256) and M = 1024, 1280 keep the staging kernel.
+static bool use_swap_kernel(int64_t m_blocks, int64_t half_n) {
+  const int64_t sms = current_sm_count();
+  const int64_t tiles_swap = m_blocks * ((half_n + 127) / 128), tiles_staged = m_blocks * ((half_n + 63) / 64);
+  if (tiles_swap < sms) return false;
+  return 9 * ((tiles_swap + sms - 1) / sms) < 5 * ((tiles_staged + sms - 1) / sms);
+}
+
 static int qbits_mm_impl(QbitsArgs& q) {
   set_kernel_family(0);
   const int64_t m = q.m, n = q.n, k = q.k;
@@ -81,27 +113,39 @@ static int qbits_mm_impl(QbitsArgs& q) {
   p.group_log2 = q.group_log2;
   p.shift_is_int = q.shift_is_int;
   const int tile_m = wgmma_tile_m(m);
-  constexpr int BN = 128;  // out-features per tile: 64 packed rows, both nibble planes
-  p.num_m_blocks = static_cast<int>((m + tile_m - 1) / tile_m);
-  p.num_n_blocks = static_cast<int>((n / 2 + BN / 2 - 1) / (BN / 2));
-  CUtensorMap ta;
+  const int64_t half_n = n / 2;
+  const int64_t m_blocks = (m + tile_m - 1) / tile_m;
+  const bool swap = use_swap_kernel(m_blocks, half_n);
+  // tile: tile_m tokens x 128 packed rows (swap-AB: both nibble planes of each) or x 64 packed rows (weight staging)
+  const int pr = swap ? 128 : 64;
+  p.num_m_blocks = static_cast<int>(m_blocks);
+  p.num_n_blocks = static_cast<int>((half_n + pr - 1) / pr);
+  CUtensorMap ta, tw;
   rc = make_tmap_2d(&ta, q.a, dtype, m, k, tile_m);
   if (rc != OK) return rc;
-  // The epilogue stores each warpgroup's 64 x 128 tile with TMA when the output is one dense, 16-byte aligned [M, N]
-  // buffer whose two nibble planes [M, 2, N/2] have 16-byte aligned rows (N % 16 == 0).  Everything else -- the fused
-  // gather's peer buffers and column slab, N % 16 != 0, a map the driver declines -- stores with ordinary stores.
+  if (swap) {
+    rc = make_tmap_packed(&tw, q.packed, half_n, k, pr);
+    if (rc != OK) return rc;
+  }
+  // The epilogue stores each warpgroup's tile with TMA when the output is one dense, 16-byte aligned [M, N] buffer whose
+  // two nibble planes [M, 2, N/2] have 16-byte aligned rows (N % 16 == 0).  Everything else -- the fused gather's peer
+  // buffers and column slab, N % 16 != 0, a map the driver declines -- stores with ordinary stores.
   CUtensorMap tout;
   std::memset(&tout, 0, sizeof(tout));
   p.epi_tma = 0;
   if (test_override(OVR_INT4_EPILOGUE) != 1 && q.g.n_out == 1 && q.g.out_peer[0] == q.out && q.ld == n && q.col0 == 0 &&
       n % 16 == 0 && reinterpret_cast<uintptr_t>(q.out) % 16 == 0) {
-    if (make_tmap_planes(&tout, q.out, dtype, m, n, 64) == OK) p.epi_tma = 1;
+    if (make_tmap_planes(&tout, q.out, dtype, m, n, swap ? tile_m : 64) == OK) p.epi_tma = 1;
     else std::memset(&tout, 0, sizeof(tout));
   }
   set_kernel_family(1);
   const bool zp = q.shift_is_int != 0;
-  if (tile_m == 64) return launch_int4<1>(ta, tout, p, dtype, zp, q.stream);
-  return launch_int4<2>(ta, tout, p, dtype, zp, q.stream);
+  if (!swap) {
+    if (tile_m == 64) return launch_int4<1>(ta, tout, p, dtype, zp, q.stream);
+    return launch_int4<2>(ta, tout, p, dtype, zp, q.stream);
+  }
+  if (tile_m == 64) return launch_w4<64>(ta, tw, tout, p, dtype, zp, q.stream);
+  return launch_w4<128>(ta, tw, tout, p, dtype, zp, q.stream);
 }
 
 }  // namespace qb

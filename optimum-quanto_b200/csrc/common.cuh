@@ -364,6 +364,88 @@ __device__ __forceinline__ void wgmma_s8_n256(uint32_t (&d)[128], uint64_t a_des
 }
 
 
+// 16-bit x 16-bit -> f32, N = NT (64 or 128), K = 16, A from REGISTERS (the 64 x 16 fragment of mma.m16n8k16 per warp:
+// a[0] row g / k 2c..2c+1, a[1] row g+8 / k 2c..2c+1, a[2] row g / k 2c+8..2c+9, a[3] row g+8 / k 2c+8..2c+9, with
+// g = lane / 4, c = lane % 4, rows offset by 16 * warp), B K-major in shared memory.  The A registers are read
+// asynchronously: they must not be written until a wgmma_wait retires the instruction.
+#define QB_WGMMA_RS_ACC32_OPERANDS                                                                                \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),      \
+      "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),       \
+      "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),      \
+      "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+#define QB_WGMMA_RS_ACC64_OPERANDS                                                                                \
+  QB_WGMMA_RS_ACC32_OPERANDS, "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]),      \
+      "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),      \
+      "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]),      \
+      "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]),      \
+      "+f"(d[62]), "+f"(d[63])
+#define QB_WGMMA_RS_LIST32                                                                                          \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                          \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}"
+#define QB_WGMMA_RS_LIST64                                                                                          \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                          \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                                  \
+  "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                                  \
+  "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+template <MmaKind KA, int NT>
+__device__ __forceinline__ void wgmma_rs(float (&d)[NT / 2], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+  static_assert(KA == MmaKind::BF16 || KA == MmaKind::F16, "register A operands are 16-bit here");
+  static_assert(NT == 64 || NT == 128, "wgmma_rs tile width");
+  if constexpr (NT == 128 && KA == MmaKind::BF16) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " QB_WGMMA_RS_LIST64
+                 ", {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n}\n"
+                 : QB_WGMMA_RS_ACC64_OPERANDS
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
+  } else if constexpr (NT == 128) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " QB_WGMMA_RS_LIST64
+                 ", {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n}\n"
+                 : QB_WGMMA_RS_ACC64_OPERANDS
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
+  } else if constexpr (KA == MmaKind::BF16) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " QB_WGMMA_RS_LIST32
+                 ", {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n}\n"
+                 : QB_WGMMA_RS_ACC32_OPERANDS
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
+  } else {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " QB_WGMMA_RS_LIST32
+                 ", {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n}\n"
+                 : QB_WGMMA_RS_ACC32_OPERANDS
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
+  }
+}
+#undef QB_WGMMA_RS_ACC32_OPERANDS
+#undef QB_WGMMA_RS_ACC64_OPERANDS
+#undef QB_WGMMA_RS_LIST32
+#undef QB_WGMMA_RS_LIST64
+
+// Four 8 x 8 16-bit matrices from the mma fragment (register q of a lane: row lane / 4, columns 2 (lane % 4), +1 of
+// matrix q) into shared memory TRANSPOSED: memory row i of matrix q (16 bytes at the address lane 8 q + i supplies)
+// receives column i of the fragment.
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
+
+// Warpgroup register reallocation: every warp of the warpgroup executes it.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// 4-byte asynchronous global -> shared copy (both addresses 4-byte aligned), and the arrive-on of an mbarrier that
+// fires once every cp.async this thread issued before it has landed (.noinc: the barrier's expected count includes it).
+__device__ __forceinline__ void cp_async_4(uint32_t smem_dst, const void* gsrc) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_dst), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint32_t bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
+}
+
 // One MMA K step (32 bytes of each operand row) of a 64-row A panel against a BN-row B tile, dispatched on the kind.
 template <MmaKind KA, int BN, typename T, int NACC>
 __device__ __forceinline__ void wgmma_step(T (&d)[NACC], uint32_t a_addr, uint32_t b_addr, uint32_t acc) {

@@ -717,4 +717,313 @@ __global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
   if (threadIdx.x == 0) gather_signal_end(p.g);  // fused all-gather: publish "this rank's slab has landed everywhere"
 }
 
+// ------------------------------------------------------------------------------------------------
+// The int4 forward, swap-AB with the dequantised weight as the REGISTER operand of wgmma:
+//
+//   out^T[n, m] = sum_k Wdeq[n, k] * x[m, k]
+//
+// A tile is PR = 128 packed rows (out-features n and n + N/2 of each) x T tokens.  Roles:
+//   warps 0-7      consumers   : warpgroup wg owns packed rows 64 wg .. 64 wg + 63 of the tile as two 64-row wgmma
+//                                fragments (f = 0, 1: rows 32 f + 8 w + g of warp w, lane 4 g + c).  Per k16 step a
+//                                thread reads its packed row's 4 bytes from shared memory, dequantises them with the
+//                                Dq arithmetic (low nibble -> fragment row g, high nibble -> row g + 8: each packed
+//                                byte feeds two rows) and issues m64 x T x k16 with A from registers and the
+//                                activations (B) from shared memory.  The next step is dequantised while the MMA runs.
+//   warp 8, lane 0 TMA producer: the activation box [T][64 k] (128B swizzle) and the packed box [PR][64 bytes] (64B
+//                                swizzle: 16-byte chunk s of row r at s ^ ((r >> 1) & 3), so the 8 rows a warp reads
+//                                per instruction hit 8 different bank groups)
+//   warp 9         coefficients: the stage's scales and shifts, as 4-byte cp.async of the aligned word holding each
+//                                value, completing on the stage's `full` barrier: no consumer waits on a global load.
+//                                (A value never straddles its aligned word, so the word lies inside the allocation.)
+//   warps 10, 11   idle        : they complete the producer warpgroup, see NTHREADS.
+// Stage shared memory: activations (A_TILE), packed bytes (W_TILE), coefficient words [set][s_lo, s_hi, z_lo, z_hi][PR]
+// (C_TILE; set 1 is the second group of a stage when the group size is 32).
+// ------------------------------------------------------------------------------------------------
+template <MmaKind KIND_, int T_, typename WT_, bool ZP_>
+struct W4Cfg {
+  static constexpr MmaKind KIND = KIND_;
+  using WT = WT_;
+  static constexpr bool ZP = ZP_;            // shift is an integer zero-point
+  static constexpr int MWG = 2;              // consumer warpgroups, 64 packed rows each
+  static constexpr int T = T_;               // token rows per tile: the wgmma N
+  static constexpr int PR = 64 * MWG;        // packed rows per tile
+  static constexpr int A_TILE = T * 128;     // activations, [T][64 k]
+  static constexpr int W_TILE = PR * 64;     // packed bytes, [PR][64 k]
+  static constexpr int C_TILE = 2 * 4 * PR * 4;
+  static constexpr int EPI_TILE = 2 * T * 128;  // per consumer warpgroup: two planes [T tokens][64 out-features]
+  static constexpr int FIT = (220 * 1024 - MWG * EPI_TILE) / (A_TILE + W_TILE + C_TILE);
+  static constexpr int NSTAGES = FIT > 8 ? 8 : FIT;
+  // full barrier: the TMA producer's arrive + the arrive-on of each lane of the coefficient warp
+  using Pipe = PipeLayout<MWG, NSTAGES, A_TILE, W_TILE + C_TILE, 0, 33, MWG * EPI_TILE>;
+  // The producer side is a whole warpgroup (TMA warp, coefficient warp, two idle warps), so that registers can move
+  // between warpgroups: each SM sub-partition's register file serves every fourth warp, and two consumer warpgroups
+  // plus one producer warp would leave 168 registers per thread -- too few to keep 128 accumulators and the A
+  // fragments of two steps, and ptxas would serialise the wgmmas.  The kernel launches at 168; with T = 128 the
+  // producer warpgroup gives back down to 56 and the consumers take 224 (64 accumulators need no more).
+  // setmaxnreg.inc waits until the CTA's pool has the registers: the two must add up to what the CTA launched with.
+  static constexpr int NTHREADS = (4 * MWG + 4) * 32;
+  static constexpr int SMEM_BYTES = Pipe::SMEM_BYTES;
+  static constexpr bool REALLOC = T == 128;
+  static constexpr int REG_CONSUMER = 224, REG_PRODUCER = 56;
+  static_assert(!REALLOC || 128 * MWG * REG_CONSUMER + 128 * REG_PRODUCER <= ((65536 / NTHREADS) & ~7) * NTHREADS,
+                "register reallocation exceeds the CTA's launch allocation");
+  static_assert(T == 64 || T == 128, "token tile");
+  static_assert(NSTAGES >= 4, "stage ring depth");
+};
+
+// Epilogue of the swap-AB kernel, one consumer warpgroup: acc[f * T/2 + 4 j + 2 h + e] is out-feature row 32 f + 8 w + g
+// of nibble plane h (packed row n_pr0 + 32 f + 8 w + g; out-feature N/2 + that for h = 1), token 8 j + 2 c + e.  The
+// rounded values go TRANSPOSED into the staging tile (two planes [T tokens][64 out-features], 128-byte rows, 128-byte
+// swizzle) with stmatrix: each 8 x 8 block of the fragment becomes 8 token rows of one 16-byte chunk.  From there the tile
+// leaves as in int4_epilogue: two TMA stores into [M, 2, N/2], or the ordinary bounds-checked copy-out.
+template <typename OT, int T>
+__device__ __forceinline__ void w4_epilogue(const GemmParams& p, const CUtensorMap* tmap_out, const float (&acc)[T],
+                                            uint32_t stile, int row0, int n_pr0, int wg) {
+  constexpr int PLANE = T * 128;
+  const int t = threadIdx.x & 127;
+  const int lane = t & 31, w = t >> 5, g = lane >> 2;
+  const int half_n = p.N / 2;
+  const OT* bias = static_cast<const OT*>(p.bias);
+  if (t == 0) bulk_wait_group_read<0>();
+  named_bar_sync(1 + wg, 128);
+  // stmatrix addresses: lane 8 q + i names token row 8 (4 jj + q) + i of matrix q; (token % 8) == i
+  const uint32_t i = static_cast<uint32_t>(lane) & 7;
+  const uint32_t lane_row = stile + ((static_cast<uint32_t>(lane) >> 3) * 8 + i) * 128;
+#pragma unroll
+  for (int f = 0; f < 2; ++f) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int n = (h ? half_n : 0) + n_pr0 + 32 * f + 8 * w + g;
+      const float b = (bias != nullptr && n < (h ? p.N : half_n)) ? to_float<OT>(bias[n]) : 0.f;
+      const uint32_t chunk = ((static_cast<uint32_t>(4 * f + w) ^ i) << 4) + h * PLANE;
+#pragma unroll
+      for (int jj = 0; jj < T / 32; ++jj) {
+        uint32_t r[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int j = 4 * jj + q;
+          float f0 = acc[f * (T / 2) + 4 * j + 2 * h], f1 = acc[f * (T / 2) + 4 * j + 2 * h + 1];
+          rnd_pair<OT>(f0, f1);
+          if (bias != nullptr) {
+            f0 = __fadd_rn(f0, b);
+            f1 = __fadd_rn(f1, b);
+            rnd_pair<OT>(f0, f1);
+          }
+          r[q] = pack2<OT>(f0, f1);
+        }
+        stmatrix_x4_trans(lane_row + jj * 32 * 128 + chunk, r[0], r[1], r[2], r[3]);
+      }
+    }
+  }
+  fence_proxy_async_smem();  // the tile's generic-proxy writes -> visible to the TMA store
+  named_bar_sync(1 + wg, 128);
+  if (p.epi_tma) {
+    if (t == 0 && row0 < p.M) {
+      tma_store_3d(tmap_out, stile, n_pr0, 0, row0);
+      tma_store_3d(tmap_out, stile + PLANE, n_pr0, 1, row0);
+      bulk_commit_group();
+    }
+    return;
+  }
+  // copy-out: thread t moves column pair 2 (t % 64) of token rows t / 64, t / 64 + 2, ...
+  const int c = 2 * (t & 63);
+  const int plane = c >> 6, pc = c & 63;
+  const int n = (plane ? half_n : 0) + n_pr0 + pc;
+  const int n_limit = plane ? p.N : half_n;
+  if (n >= n_limit) return;
+  const bool two = n + 1 < n_limit;
+  const uint32_t src = stile + plane * PLANE + (pc & 7) * 2;
+  for (int r = t >> 6; r < T && row0 + r < p.M; r += 2) {
+    const uint32_t v = ld_shared_u32(src + r * 128 + ((static_cast<uint32_t>(pc >> 3) ^ (r & 7)) << 4));
+    const size_t off = static_cast<size_t>(row0 + r) * p.ld + p.col0 + n;
+    const bool vec = (off * sizeof(OT)) % (2 * sizeof(OT)) == 0;
+    for (int q = 0; q < p.g.n_out; ++q) {
+      uint16_t* dst = static_cast<uint16_t*>(p.g.out_peer[q]) + off;
+      if (two && vec) {
+        *reinterpret_cast<uint32_t*>(dst) = v;
+      } else {
+        dst[0] = static_cast<uint16_t>(v);
+        if (two) dst[1] = static_cast<uint16_t>(v >> 16);
+      }
+    }
+  }
+}
+
+// the aligned 4-byte word that holds byte `off` of `base`, and the bit position of that byte in it
+__device__ __forceinline__ const void* word_of(const void* base, size_t off) {
+  return reinterpret_cast<const void*>((reinterpret_cast<uintptr_t>(base) + off) & ~static_cast<uintptr_t>(3));
+}
+__device__ __forceinline__ uint32_t bitpos_of(const void* base, size_t off) {
+  return static_cast<uint32_t>((reinterpret_cast<uintptr_t>(base) + off) & 3) * 8;
+}
+
+// keeps the compiler from moving writes of a wgmma A fragment above the wgmma_wait that frees its registers
+__device__ __forceinline__ void fence_frag(uint32_t (&a)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(a[i])::"memory");
+}
+
+template <class Cfg>
+__global__ void __launch_bounds__(Cfg::NTHREADS, 1)
+    gemm_w4_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
+                   const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
+  using L = typename Cfg::Pipe;
+  using WT = typename Cfg::WT;
+  using D = Dq<WT>;
+  constexpr int T = Cfg::T, PR = Cfg::PR;
+  constexpr bool ZP = Cfg::ZP;
+
+  const auto pipe = WgmmaPipe<L>::init([&] {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_w);
+    if (p.epi_tma) tma_prefetch_desc(&tmap_out);
+  });
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
+  const int kblocks = (p.K + 63) / 64;
+  const int half_n = p.N / 2;
+  const int gpr = p.K / p.group;       // groups per out-feature row
+  const bool two_sets = p.group < 64;  // group size 32: two (scale, shift) sets per 64-k stage
+
+  if (warp < L::PRODUCER_WARP) {
+    // ------------------------------------------------------------------ consumers: dequantise + wgmma + epilogue
+    if constexpr (Cfg::REALLOC) setmaxnreg_inc<Cfg::REG_CONSUMER>();
+    const int wg = warp >> 2;
+    const int g = lane >> 2, c = lane & 3;
+    const int r0 = 64 * wg + 8 * (warp & 3) + g;  // this thread's packed row of fragment 0 in the tile (+32: fragment 1)
+    uint32_t roff[2], rsw[2];
+#pragma unroll
+    for (int f = 0; f < 2; ++f) {
+      const uint32_t r = static_cast<uint32_t>(r0 + 32 * f);
+      roff[f] = r * 64 + 4 * (static_cast<uint32_t>(c) >> 1);  // word c / 2 of a chunk holds k 2c, 2c+1; word 2 + c / 2 k 2c+8, 2c+9
+      rsw[f] = (r >> 1) & 3;
+    }
+    const uint32_t sel = (c & 1) ? 0x7632u : 0x5410u;
+    float acc[T];
+    RingPos<L::NSTAGES> pos;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int m_blk = tile % p.num_m_blocks;
+      const int n_blk = tile / p.num_m_blocks;
+      const int rp0 = n_blk * PR + r0;
+      int kb = 0;
+      // byte position (mod 4) of group 0 of s_lo, s_hi, z_lo, z_hi of fragment f's packed row inside its aligned word
+      uint32_t cb[2][4];
+#pragma unroll
+      for (int f = 0; f < 2; ++f) {
+        const size_t ilo = static_cast<size_t>(rp0 + 32 * f) * gpr;
+        const size_t ihi = ilo + static_cast<size_t>(half_n) * gpr;
+        cb[f][0] = bitpos_of(p.wscale, 2 * ilo) >> 3;
+        cb[f][1] = bitpos_of(p.wscale, 2 * ihi) >> 3;
+        cb[f][2] = bitpos_of(p.wshift, (ZP ? 1 : 2) * ilo) >> 3;
+        cb[f][3] = bitpos_of(p.wshift, (ZP ? 1 : 2) * ihi) >> 3;
+      }
+      // (scale, shift) of both nibbles of fragment f's packed row for coefficient set `set` of the stage at k `kset`
+      auto coefs = [&](uint32_t ct, int set, int kset, typename D::Coef (&klo)[2], typename D::Coef (&khi)[2]) {
+        const uint32_t grp = static_cast<uint32_t>((p.group_log2 >= 0) ? (kset >> p.group_log2) : (kset / p.group));
+        const uint32_t gs = 2 * grp, gz = (ZP ? 1 : 2) * grp;
+#pragma unroll
+        for (int f = 0; f < 2; ++f) {
+          const uint32_t a = ct + static_cast<uint32_t>(set * 4 * PR + r0 + 32 * f) * 4;
+          const uint16_t s_lo = static_cast<uint16_t>(ld_shared_u32(a) >> (((cb[f][0] + gs) & 3) << 3));
+          const uint16_t s_hi = static_cast<uint16_t>(ld_shared_u32(a + PR * 4) >> (((cb[f][1] + gs) & 3) << 3));
+          uint16_t z_lo = static_cast<uint16_t>(ld_shared_u32(a + 2 * PR * 4) >> (((cb[f][2] + gz) & 3) << 3));
+          uint16_t z_hi = static_cast<uint16_t>(ld_shared_u32(a + 3 * PR * 4) >> (((cb[f][3] + gz) & 3) << 3));
+          if (ZP) {
+            z_lo &= 0xFF;
+            z_hi &= 0xFF;
+          }
+          klo[f] = D::make_raw(bits_as<WT>(s_lo), z_lo, ZP);
+          khi[f] = D::make_raw(bits_as<WT>(s_hi), z_hi, ZP);
+        }
+      };
+      pipe.consume_tile(pos, kblocks, acc, [&](uint32_t, uint32_t wt, bool accumulate) {
+        const uint32_t act = wt - Cfg::A_TILE, ct = wt + Cfg::W_TILE;
+        const int kbase = 64 * kb++;
+        // steps 2 and 3 read set 1 with groups of 32, except in a K tail (K % 64 == 32) where their activations are zero
+        // and set 0 stands in (no branch between the wgmma groups: set 0 is simply read again)
+        const int set2 = (two_sets && kbase + 32 < p.K) ? 1 : 0;
+        typename D::Coef klo[2], khi[2];
+        coefs(ct, 0, kbase, klo, khi);
+        uint32_t a[2][2][4];  // [step parity][fragment]: the registers of the step in flight stay untouched
+#pragma unroll
+        for (int st = 0; st < 4; ++st) {
+          if (st == 2) coefs(ct, set2, kbase + 32 * set2, klo, khi);
+#pragma unroll
+          for (int f = 0; f < 2; ++f) {
+            uint32_t (&af)[4] = a[st & 1][f];
+            fence_frag(af);
+            const uint32_t chunk = wt + roff[f] + ((static_cast<uint32_t>(st) ^ rsw[f]) << 4);
+            const uint32_t x = __byte_perm(ld_shared_u32(chunk), ld_shared_u32(chunk + 8), sel);
+            const uint32_t wl = x & 0x0F0F0F0Fu, wh = (x >> 4) & 0x0F0F0F0Fu;
+            af[0] = D::cvt(__byte_perm(wl, D::MAGIC_BYTES, 0x4140), klo[f], ZP);  // row g,     k 2c, 2c+1
+            af[1] = D::cvt(__byte_perm(wh, D::MAGIC_BYTES, 0x4140), khi[f], ZP);  // row g + 8, k 2c, 2c+1
+            af[2] = D::cvt(__byte_perm(wl, D::MAGIC_BYTES, 0x4342), klo[f], ZP);  // row g,     k 2c+8, 2c+9
+            af[3] = D::cvt(__byte_perm(wh, D::MAGIC_BYTES, 0x4342), khi[f], ZP);  // row g + 8, k 2c+8, 2c+9
+          }
+          wgmma_fence();
+          const uint64_t db = wgmma_desc_sw128(act + st * 32);
+#pragma unroll
+          for (int f = 0; f < 2; ++f)
+            wgmma_rs<Cfg::KIND, T>(*reinterpret_cast<float(*)[T / 2]>(acc + f * (T / 2)), a[st & 1][f], db,
+                                   (st > 0 || accumulate) ? 1u : 0u);
+          // the last step is committed by consume_tile, whose wait retires step 2 before the next stage writes its set
+          if (st < 3) {
+            wgmma_commit();
+            wgmma_wait<1>();  // retires step st - 1: its registers take step st + 1
+          }
+        }
+      });
+      w4_epilogue<WT, T>(p, &tmap_out, acc, pipe.epi + wg * Cfg::EPI_TILE, m_blk * T, n_blk * PR + 64 * wg, wg);
+    }
+    if ((threadIdx.x & 127) == 0) bulk_wait_group_all();  // the last tile's TMA store has completed
+    if (p.g.n_out > 1) __threadfence_system();            // this thread's peer stores are performed before the rank signals
+  } else {
+    if constexpr (Cfg::REALLOC) setmaxnreg_dec<Cfg::REG_PRODUCER>();
+    if (warp == L::PRODUCER_WARP && lane == 0) {
+      // ---------------------------------------------------------------- TMA producer: activations + packed bytes
+      gather_wait_start(p.g);  // the activation may be the gathered output of the previous linear
+      pipe.produce(num_tiles, p.num_m_blocks, kblocks, Cfg::A_TILE + Cfg::W_TILE,
+                   [&](uint8_t* dst, uint64_t* bar, int m_blk, int n_blk, int kb) {
+                     tma_load_2d(dst, &tmap_a, bar, kb * 64, m_blk * T);
+                     tma_load_2d(dst + Cfg::A_TILE, &tmap_w, bar, kb * 64, n_blk * PR);
+                   });
+    } else if (warp == L::PRODUCER_WARP + 1) {
+      // ---------------------------------------------------------------- the stages' scales and shifts
+      constexpr size_t ZB = ZP ? 1 : 2;  // bytes per shift
+      const int nsets = two_sets ? 2 : 1;
+      RingPos<L::NSTAGES> pos;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int n_blk = tile / p.num_m_blocks;
+        for (int kb = 0; kb < kblocks; ++kb) {
+          mbar_wait(&pipe.empty_bar[pos.stage], pos.phase ^ 1u);
+          const uint32_t ct = pipe.b_addr(pos.stage) + Cfg::W_TILE;
+          const int kbase = 64 * kb;
+          const int g0 = (p.group_log2 >= 0) ? (kbase >> p.group_log2) : (kbase / p.group);
+          for (int e = lane; e < nsets * PR; e += 32) {
+            const int set = e >= PR ? 1 : 0;
+            const int row = e - set * PR;
+            const int rp = n_blk * PR + row;
+            // rows past N/2 are never stored; a K-tail second group (K % 64 == 32) is never read
+            if (rp >= half_n || (set == 1 && kbase + 32 >= p.K)) continue;
+            const size_t ilo = static_cast<size_t>(rp) * gpr + g0 + set;
+            const size_t ihi = ilo + static_cast<size_t>(half_n) * gpr;
+            const uint32_t d = ct + static_cast<uint32_t>(set * 4 * PR + row) * 4;
+            cp_async_4(d, word_of(p.wscale, 2 * ilo));
+            cp_async_4(d + PR * 4, word_of(p.wscale, 2 * ihi));
+            cp_async_4(d + 2 * PR * 4, word_of(p.wshift, ZB * ilo));
+            cp_async_4(d + 3 * PR * 4, word_of(p.wshift, ZB * ihi));
+          }
+          cp_async_mbar_arrive_noinc(smem_u32(&pipe.full_bar[pos.stage]));
+          pos.advance();
+        }
+      }
+    }
+  }
+
+  __syncthreads();
+  if (threadIdx.x == 0) gather_signal_end(p.g);  // fused all-gather: publish "this rank's slab has landed everywhere"
+}
+
 }  // namespace qb

@@ -74,6 +74,9 @@ int make_tmap_2d(CUtensorMap* map, const void* base, int dt, int64_t rows, int64
 // Row-major [rows, cols] 16-bit matrix described as [rows, 2, cols/2] (two column planes); box = 64 elements of one
 // plane x box_rows rows, 128-byte swizzle.  A box never crosses cols/2: past the end of a plane TMA fills zeros.
 int make_tmap_planes(CUtensorMap* map, const void* base, int dt, int64_t rows, int64_t cols, int box_rows);
+// Packed int4 weights [rows, cols] bytes; box = 64 bytes of a row x box_rows rows, 64-byte swizzle (16-byte chunk s of
+// row r at chunk s ^ ((r >> 1) & 3)).
+int make_tmap_packed(CUtensorMap* map, const uint8_t* packed, int64_t rows, int64_t cols, int box_rows);
 // [rows, cols] view with an explicit row pitch and box: the epilogue's TMA stores into (a column slab of) the output.
 int make_tmap_2d_view(CUtensorMap* map, const void* base, int dt, int64_t rows, int64_t cols, int64_t pitch_elems,
                       int box_cols, int box_rows, bool swizzle128);
