@@ -52,16 +52,33 @@ static int launch_w4(const CUtensorMap& ta, const CUtensorMap& tw, const CUtenso
   return launch_persistent<gemm_w4_kernel<C>, C>(tiles, st, "gemm_w4_kernel launch", ta, tw, tout, p);
 }
 
-// Which int4 wgmma kernel runs a problem of m_blocks token tiles and half_n packed rows.  The swap-AB kernel
-// (gemm_w4_kernel) does a tile of 128 packed rows in about 1.8x the time the weight-staging kernel (gemm_tc_kernel)
-// takes for its 64-row tile (H100 SXM, bf16, M = 4096: 1.10 vs 1.22 ms for twice the tiles), so it wins once its tiles
-// fill every SM and its waves, 1.8x as long, are fewer than 5/9 of the staging kernel's.  At N = 14336 on 132 SMs that
-// is M = 512, 768 and M >= 1536; small batches (M <= 256) and M = 1024, 1280 keep the staging kernel.
+// Which int4 wgmma kernel runs a problem of m_blocks 128-token blocks and half_n packed rows.  The swap-AB kernel
+// (gemm_w4_kernel) was measured on tiles of 128 tokens x 128 packed rows, the same MACs as its 256 x 64 tiles: such a
+// tile took about 1.8x the time the weight-staging kernel (gemm_tc_kernel) takes for its 128 x 64 tile (H100 SXM, bf16,
+// M = 4096: 1.10 vs 1.22 ms for twice the tiles), so it wins once its tiles fill every SM and its waves, 1.8x as long,
+// are fewer than 5/9 of the staging kernel's.  At N = 14336 on 132 SMs that is M = 512, 768 and M >= 1536; small batches
+// (M <= 256) and M = 1024, 1280 keep the staging kernel.
 static bool use_swap_kernel(int64_t m_blocks, int64_t half_n) {
   const int64_t sms = current_sm_count();
   const int64_t tiles_swap = m_blocks * ((half_n + 127) / 128), tiles_staged = m_blocks * ((half_n + 63) / 64);
   if (tiles_swap < sms) return false;
   return 9 * ((tiles_swap + sms - 1) / sms) < 5 * ((tiles_staged + sms - 1) / sms);
+}
+
+// Token rows per tile of the swap-AB kernel: 64 while M <= 64; else 256 where the 256 x 64 tiles cost less than the
+// 128 x 128 ones, else 128.  Both tile sizes cover the same packed rows per token, so the costs compare as the tokens
+// the tiles span (M rounded up to the tile) times the time per token row: 0.72-0.77 as much at T = 256 (H100 SXM, bf16,
+// N = 14336, K = 4096: 0.755 vs 0.980 ms at M = 4096, 0.111 vs 0.151 at M = 512, 0.408 vs 0.566 at M = 2048), taken
+// as 3/4.  So M <= 128 keeps 128-token tiles (a 256-token tile would be more than half empty), and so does a ragged
+// M = 256 j + r with 0 < r <= 128 while j is small (M = 257 ... 384: 512 tokens against 384).  use_swap_kernel counts
+// 128 x 128 tiles: the tile chosen here is, by this estimate, no slower than those.  Test override OVR_TILE_M forces 64,
+// 128 or 256.
+static int swap_tile_t(int64_t m) {
+  const int force = test_override(OVR_TILE_M);
+  if (force == 64 || force == 128 || force == 256) return force;
+  if (m <= 64) return 64;
+  const int64_t span256 = (m + 255) / 256 * 256, span128 = (m + 127) / 128 * 128;
+  return 3 * span256 < 4 * span128 ? 256 : 128;
 }
 
 static int qbits_mm_impl(QbitsArgs& q) {
@@ -114,14 +131,17 @@ static int qbits_mm_impl(QbitsArgs& q) {
   p.shift_is_int = q.shift_is_int;
   const int tile_m = wgmma_tile_m(m);
   const int64_t half_n = n / 2;
-  const int64_t m_blocks = (m + tile_m - 1) / tile_m;
-  const bool swap = use_swap_kernel(m_blocks, half_n);
-  // tile: tile_m tokens x 128 packed rows (swap-AB: both nibble planes of each) or x 64 packed rows (weight staging)
-  const int pr = swap ? 128 : 64;
+  // OVR_TILE_M = 256 names the swap-AB kernel's 256-token tile, at any shape
+  const bool swap = test_override(OVR_TILE_M) == 256 || use_swap_kernel((m + tile_m - 1) / tile_m, half_n);
+  // tile: t tokens x pr packed rows (swap-AB: both nibble planes of each; 64 and 128 tokens go with 128 packed rows,
+  // 256 tokens with 64) or x 64 packed rows (weight staging)
+  const int t = swap ? swap_tile_t(m) : tile_m;
+  const int pr = (swap && t != 256) ? 128 : 64;
+  const int64_t m_blocks = (m + t - 1) / t;
   p.num_m_blocks = static_cast<int>(m_blocks);
   p.num_n_blocks = static_cast<int>((half_n + pr - 1) / pr);
   CUtensorMap ta, tw;
-  rc = make_tmap_2d(&ta, q.a, dtype, m, k, tile_m);
+  rc = make_tmap_2d(&ta, q.a, dtype, m, k, t);
   if (rc != OK) return rc;
   if (swap) {
     rc = make_tmap_packed(&tw, q.packed, half_n, k, pr);
@@ -135,7 +155,7 @@ static int qbits_mm_impl(QbitsArgs& q) {
   p.epi_tma = 0;
   if (test_override(OVR_INT4_EPILOGUE) != 1 && q.g.n_out == 1 && q.g.out_peer[0] == q.out && q.ld == n && q.col0 == 0 &&
       n % 16 == 0 && reinterpret_cast<uintptr_t>(q.out) % 16 == 0) {
-    if (make_tmap_planes(&tout, q.out, dtype, m, n, swap ? tile_m : 64) == OK) p.epi_tma = 1;
+    if (make_tmap_planes(&tout, q.out, dtype, m, n, swap ? t : 64) == OK) p.epi_tma = 1;
     else std::memset(&tout, 0, sizeof(tout));
   }
   set_kernel_family(1);
@@ -144,8 +164,9 @@ static int qbits_mm_impl(QbitsArgs& q) {
     if (tile_m == 64) return launch_int4<1>(ta, tout, p, dtype, zp, q.stream);
     return launch_int4<2>(ta, tout, p, dtype, zp, q.stream);
   }
-  if (tile_m == 64) return launch_w4<64>(ta, tw, tout, p, dtype, zp, q.stream);
-  return launch_w4<128>(ta, tw, tout, p, dtype, zp, q.stream);
+  if (t == 64) return launch_w4<64>(ta, tw, tout, p, dtype, zp, q.stream);
+  if (t == 128) return launch_w4<128>(ta, tw, tout, p, dtype, zp, q.stream);
+  return launch_w4<256>(ta, tw, tout, p, dtype, zp, q.stream);
 }
 
 }  // namespace qb

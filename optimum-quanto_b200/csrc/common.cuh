@@ -364,7 +364,7 @@ __device__ __forceinline__ void wgmma_s8_n256(uint32_t (&d)[128], uint64_t a_des
 }
 
 
-// 16-bit x 16-bit -> f32, N = NT (64 or 128), K = 16, A from REGISTERS (the 64 x 16 fragment of mma.m16n8k16 per warp:
+// 16-bit x 16-bit -> f32, N = NT (64, 128 or 256), K = 16, A from REGISTERS (the 64 x 16 fragment of mma.m16n8k16 per warp:
 // a[0] row g / k 2c..2c+1, a[1] row g+8 / k 2c..2c+1, a[2] row g / k 2c+8..2c+9, a[3] row g+8 / k 2c+8..2c+9, with
 // g = lane / 4, c = lane % 4, rows offset by 16 * warp), B K-major in shared memory.  The A registers are read
 // asynchronously: they must not be written until a wgmma_wait retires the instruction.
@@ -387,11 +387,42 @@ __device__ __forceinline__ void wgmma_s8_n256(uint32_t (&d)[128], uint64_t a_des
   "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                                  \
   "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                                  \
   "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define QB_WGMMA_RS_ACC128_OPERANDS                                                                               \
+  QB_WGMMA_RS_ACC64_OPERANDS, "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]),      \
+      "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]),      \
+      "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]),      \
+      "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]),      \
+      "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]),    \
+      "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]),            \
+      "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]),            \
+      "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]),            \
+      "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+#define QB_WGMMA_RS_LIST128                                                                                         \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                          \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                                  \
+  "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                                  \
+  "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "                                  \
+  "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "                                  \
+  "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "                                  \
+  "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "                      \
+  "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}"
 template <MmaKind KA, int NT>
 __device__ __forceinline__ void wgmma_rs(float (&d)[NT / 2], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
   static_assert(KA == MmaKind::BF16 || KA == MmaKind::F16, "register A operands are 16-bit here");
-  static_assert(NT == 64 || NT == 128, "wgmma_rs tile width");
-  if constexpr (NT == 128 && KA == MmaKind::BF16) {
+  static_assert(NT == 64 || NT == 128 || NT == 256, "wgmma_rs tile width");
+  if constexpr (NT == 256 && KA == MmaKind::BF16) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %133, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 " QB_WGMMA_RS_LIST128
+                 ", {%128, %129, %130, %131}, %132, p, 1, 1, 0;\n}\n"
+                 : QB_WGMMA_RS_ACC128_OPERANDS
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
+  } else if constexpr (NT == 256) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %133, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 " QB_WGMMA_RS_LIST128
+                 ", {%128, %129, %130, %131}, %132, p, 1, 1, 0;\n}\n"
+                 : QB_WGMMA_RS_ACC128_OPERANDS
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
+  } else if constexpr (NT == 128 && KA == MmaKind::BF16) {
     asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
                  "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " QB_WGMMA_RS_LIST64
                  ", {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n}\n"
@@ -421,6 +452,8 @@ __device__ __forceinline__ void wgmma_rs(float (&d)[NT / 2], const uint32_t (&a)
 #undef QB_WGMMA_RS_ACC64_OPERANDS
 #undef QB_WGMMA_RS_LIST32
 #undef QB_WGMMA_RS_LIST64
+#undef QB_WGMMA_RS_ACC128_OPERANDS
+#undef QB_WGMMA_RS_LIST128
 
 // Four 8 x 8 16-bit matrices from the mma fragment (register q of a lane: row lane / 4, columns 2 (lane % 4), +1 of
 // matrix q) into shared memory TRANSPOSED: memory row i of matrix q (16 bytes at the address lane 8 q + i supplies)

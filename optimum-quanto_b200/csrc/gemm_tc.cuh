@@ -722,9 +722,11 @@ __global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
 //
 //   out^T[n, m] = sum_k Wdeq[n, k] * x[m, k]
 //
-// A tile is PR = 128 packed rows (out-features n and n + N/2 of each) x T tokens.  Roles:
-//   warps 0-7      consumers   : warpgroup wg owns packed rows 64 wg .. 64 wg + 63 of the tile as two 64-row wgmma
-//                                fragments (f = 0, 1: rows 32 f + 8 w + g of warp w, lane 4 g + c).  Per k16 step a
+// A tile is PR packed rows (out-features n and n + N/2 of each) x T tokens: PR = 128 at T = 64 and 128, PR = 64 at
+// T = 256 (the MACs of T = 128; one m64n256k16 per step takes the dequantised values two m64n128k16 took).
+// Roles:
+//   warps 0-7      consumers   : warpgroup wg owns NF 64-row wgmma fragments (NF = 1 at T = 256, else 2), fragment
+//                                f = packed rows 32 (NF wg + f) + 8 w + g of warp w, lane 4 g + c.  Per k16 step a
 //                                thread reads its packed row's 4 bytes from shared memory, dequantises them with the
 //                                Dq arithmetic (low nibble -> fragment row g, high nibble -> row g + 8: each packed
 //                                byte feeds two rows) and issues m64 x T x k16 with A from registers and the
@@ -744,58 +746,66 @@ struct W4Cfg {
   static constexpr MmaKind KIND = KIND_;
   using WT = WT_;
   static constexpr bool ZP = ZP_;            // shift is an integer zero-point
-  static constexpr int MWG = 2;              // consumer warpgroups, 64 packed rows each
+  static constexpr int MWG = 2;              // consumer warpgroups
   static constexpr int T = T_;               // token rows per tile: the wgmma N
-  static constexpr int PR = 64 * MWG;        // packed rows per tile
+  static constexpr int NF = T == 256 ? 1 : 2;  // 64-row fragments (32 packed rows) per consumer warpgroup
+  static constexpr int PR = 32 * NF * MWG;   // packed rows per tile
   static constexpr int A_TILE = T * 128;     // activations, [T][64 k]
   static constexpr int W_TILE = PR * 64;     // packed bytes, [PR][64 k]
   static constexpr int C_TILE = 2 * 4 * PR * 4;
-  static constexpr int EPI_TILE = 2 * T * 128;  // per consumer warpgroup: two planes [T tokens][64 out-features]
-  static constexpr int FIT = (220 * 1024 - MWG * EPI_TILE) / (A_TILE + W_TILE + C_TILE);
+  // output staging, one tile per 64 packed rows: two planes [T tokens][64 out-features]
+  static constexpr int EPI_TILE = 2 * T * 128;
+  static constexpr int EPI_BYTES = (PR / 64) * EPI_TILE;
+  static constexpr int FIT = (220 * 1024 - EPI_BYTES) / (A_TILE + W_TILE + C_TILE);
   static constexpr int NSTAGES = FIT > 8 ? 8 : FIT;
   // full barrier: the TMA producer's arrive + the arrive-on of each lane of the coefficient warp
-  using Pipe = PipeLayout<MWG, NSTAGES, A_TILE, W_TILE + C_TILE, 0, 33, MWG * EPI_TILE>;
+  using Pipe = PipeLayout<MWG, NSTAGES, A_TILE, W_TILE + C_TILE, 0, 33, EPI_BYTES>;
   // The producer side is a whole warpgroup (TMA warp, coefficient warp, two idle warps), so that registers can move
   // between warpgroups: each SM sub-partition's register file serves every fourth warp, and two consumer warpgroups
   // plus one producer warp would leave 168 registers per thread -- too few to keep 128 accumulators and the A
-  // fragments of two steps, and ptxas would serialise the wgmmas.  The kernel launches at 168; with T = 128 the
+  // fragments of two steps, and ptxas would serialise the wgmmas.  The kernel launches at 168; with T >= 128 the
   // producer warpgroup gives back down to 56 and the consumers take 224 (64 accumulators need no more).
   // setmaxnreg.inc waits until the CTA's pool has the registers: the two must add up to what the CTA launched with.
   static constexpr int NTHREADS = (4 * MWG + 4) * 32;
   static constexpr int SMEM_BYTES = Pipe::SMEM_BYTES;
-  static constexpr bool REALLOC = T == 128;
+  static constexpr bool REALLOC = T >= 128;
   static constexpr int REG_CONSUMER = 224, REG_PRODUCER = 56;
   static_assert(!REALLOC || 128 * MWG * REG_CONSUMER + 128 * REG_PRODUCER <= ((65536 / NTHREADS) & ~7) * NTHREADS,
                 "register reallocation exceeds the CTA's launch allocation");
-  static_assert(T == 64 || T == 128, "token tile");
+  static_assert(T == 64 || T == 128 || T == 256, "token tile");
   static_assert(NSTAGES >= 4, "stage ring depth");
 };
 
-// Epilogue of the swap-AB kernel, one consumer warpgroup: acc[f * T/2 + 4 j + 2 h + e] is out-feature row 32 f + 8 w + g
-// of nibble plane h (packed row n_pr0 + 32 f + 8 w + g; out-feature N/2 + that for h = 1), token 8 j + 2 c + e.  The
-// rounded values go TRANSPOSED into the staging tile (two planes [T tokens][64 out-features], 128-byte rows, 128-byte
-// swizzle) with stmatrix: each 8 x 8 block of the fragment becomes 8 token rows of one 16-byte chunk.  From there the tile
-// leaves as in int4_epilogue: two TMA stores into [M, 2, N/2], or the ordinary bounds-checked copy-out.
-template <typename OT, int T>
-__device__ __forceinline__ void w4_epilogue(const GemmParams& p, const CUtensorMap* tmap_out, const float (&acc)[T],
-                                            uint32_t stile, int row0, int n_pr0, int wg) {
+// Epilogue of the swap-AB kernel, the threads that share one staging tile (64 packed rows: one consumer warpgroup when
+// NF = 2, both when NF = 1).  acc[f * T/2 + 4 j + 2 h + e] is out-feature row 32 fc + 8 w + g of the staging tile
+// (fc = f, or wg when NF = 1) of nibble plane h (packed row n_pr0 + that; out-feature N/2 + that for h = 1), token
+// 8 j + 2 c + e.  The rounded values go TRANSPOSED into the staging tile (two planes [T tokens][64 out-features],
+// 128-byte rows, 128-byte swizzle) with stmatrix: each 8 x 8 block of the fragment becomes 8 token rows of one 16-byte
+// chunk.  From there the tile leaves as in int4_epilogue: two TMA stores into [M, 2, N/2], or the ordinary
+// bounds-checked copy-out.
+template <typename OT, int T, int NF>
+__device__ __forceinline__ void w4_epilogue(const GemmParams& p, const CUtensorMap* tmap_out,
+                                            const float (&acc)[NF * T / 2], uint32_t stile, int row0, int n_pr0, int wg) {
   constexpr int PLANE = T * 128;
-  const int t = threadIdx.x & 127;
-  const int lane = t & 31, w = t >> 5, g = lane >> 2;
+  constexpr int ET = NF == 1 ? 256 : 128;  // threads of the staging tile
+  const int bar = NF == 1 ? 1 : 1 + wg;
+  const int t = static_cast<int>(threadIdx.x) & (ET - 1);
+  const int lane = t & 31, w = (t >> 5) & 3, g = lane >> 2;
   const int half_n = p.N / 2;
   const OT* bias = static_cast<const OT*>(p.bias);
   if (t == 0) bulk_wait_group_read<0>();
-  named_bar_sync(1 + wg, 128);
+  named_bar_sync(bar, ET);
   // stmatrix addresses: lane 8 q + i names token row 8 (4 jj + q) + i of matrix q; (token % 8) == i
   const uint32_t i = static_cast<uint32_t>(lane) & 7;
   const uint32_t lane_row = stile + ((static_cast<uint32_t>(lane) >> 3) * 8 + i) * 128;
 #pragma unroll
-  for (int f = 0; f < 2; ++f) {
+  for (int f = 0; f < NF; ++f) {
+    const int fc = NF == 1 ? wg : f;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int n = (h ? half_n : 0) + n_pr0 + 32 * f + 8 * w + g;
+      const int n = (h ? half_n : 0) + n_pr0 + 32 * fc + 8 * w + g;
       const float b = (bias != nullptr && n < (h ? p.N : half_n)) ? to_float<OT>(bias[n]) : 0.f;
-      const uint32_t chunk = ((static_cast<uint32_t>(4 * f + w) ^ i) << 4) + h * PLANE;
+      const uint32_t chunk = ((static_cast<uint32_t>(4 * fc + w) ^ i) << 4) + h * PLANE;
 #pragma unroll
       for (int jj = 0; jj < T / 32; ++jj) {
         uint32_t r[4];
@@ -816,7 +826,7 @@ __device__ __forceinline__ void w4_epilogue(const GemmParams& p, const CUtensorM
     }
   }
   fence_proxy_async_smem();  // the tile's generic-proxy writes -> visible to the TMA store
-  named_bar_sync(1 + wg, 128);
+  named_bar_sync(bar, ET);
   if (p.epi_tma) {
     if (t == 0 && row0 < p.M) {
       tma_store_3d(tmap_out, stile, n_pr0, 0, row0);
@@ -825,7 +835,7 @@ __device__ __forceinline__ void w4_epilogue(const GemmParams& p, const CUtensorM
     }
     return;
   }
-  // copy-out: thread t moves column pair 2 (t % 64) of token rows t / 64, t / 64 + 2, ...
+  // copy-out: thread t moves column pair 2 (t % 64) of token rows t / 64, t / 64 + ET / 64, ...
   const int c = 2 * (t & 63);
   const int plane = c >> 6, pc = c & 63;
   const int n = (plane ? half_n : 0) + n_pr0 + pc;
@@ -833,7 +843,7 @@ __device__ __forceinline__ void w4_epilogue(const GemmParams& p, const CUtensorM
   if (n >= n_limit) return;
   const bool two = n + 1 < n_limit;
   const uint32_t src = stile + plane * PLANE + (pc & 7) * 2;
-  for (int r = t >> 6; r < T && row0 + r < p.M; r += 2) {
+  for (int r = t >> 6; r < T && row0 + r < p.M; r += ET / 64) {
     const uint32_t v = ld_shared_u32(src + r * 128 + ((static_cast<uint32_t>(pc >> 3) ^ (r & 7)) << 4));
     const size_t off = static_cast<size_t>(row0 + r) * p.ld + p.col0 + n;
     const bool vec = (off * sizeof(OT)) % (2 * sizeof(OT)) == 0;
@@ -870,7 +880,7 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
   using L = typename Cfg::Pipe;
   using WT = typename Cfg::WT;
   using D = Dq<WT>;
-  constexpr int T = Cfg::T, PR = Cfg::PR;
+  constexpr int T = Cfg::T, PR = Cfg::PR, NF = Cfg::NF;
   constexpr bool ZP = Cfg::ZP;
 
   const auto pipe = WgmmaPipe<L>::init([&] {
@@ -892,16 +902,16 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
     if constexpr (Cfg::REALLOC) setmaxnreg_inc<Cfg::REG_CONSUMER>();
     const int wg = warp >> 2;
     const int g = lane >> 2, c = lane & 3;
-    const int r0 = 64 * wg + 8 * (warp & 3) + g;  // this thread's packed row of fragment 0 in the tile (+32: fragment 1)
-    uint32_t roff[2], rsw[2];
+    const int r0 = 32 * NF * wg + 8 * (warp & 3) + g;  // this thread's packed row of fragment 0 in the tile (+32: fragment 1)
+    uint32_t roff[NF], rsw[NF];
 #pragma unroll
-    for (int f = 0; f < 2; ++f) {
+    for (int f = 0; f < NF; ++f) {
       const uint32_t r = static_cast<uint32_t>(r0 + 32 * f);
       roff[f] = r * 64 + 4 * (static_cast<uint32_t>(c) >> 1);  // word c / 2 of a chunk holds k 2c, 2c+1; word 2 + c / 2 k 2c+8, 2c+9
       rsw[f] = (r >> 1) & 3;
     }
     const uint32_t sel = (c & 1) ? 0x7632u : 0x5410u;
-    float acc[T];
+    float acc[NF * T / 2];
     RingPos<L::NSTAGES> pos;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m_blk = tile % p.num_m_blocks;
@@ -909,9 +919,9 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
       const int rp0 = n_blk * PR + r0;
       int kb = 0;
       // byte position (mod 4) of group 0 of s_lo, s_hi, z_lo, z_hi of fragment f's packed row inside its aligned word
-      uint32_t cb[2][4];
+      uint32_t cb[NF][4];
 #pragma unroll
-      for (int f = 0; f < 2; ++f) {
+      for (int f = 0; f < NF; ++f) {
         const size_t ilo = static_cast<size_t>(rp0 + 32 * f) * gpr;
         const size_t ihi = ilo + static_cast<size_t>(half_n) * gpr;
         cb[f][0] = bitpos_of(p.wscale, 2 * ilo) >> 3;
@@ -920,11 +930,11 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
         cb[f][3] = bitpos_of(p.wshift, (ZP ? 1 : 2) * ihi) >> 3;
       }
       // (scale, shift) of both nibbles of fragment f's packed row for coefficient set `set` of the stage at k `kset`
-      auto coefs = [&](uint32_t ct, int set, int kset, typename D::Coef (&klo)[2], typename D::Coef (&khi)[2]) {
+      auto coefs = [&](uint32_t ct, int set, int kset, typename D::Coef (&klo)[NF], typename D::Coef (&khi)[NF]) {
         const uint32_t grp = static_cast<uint32_t>((p.group_log2 >= 0) ? (kset >> p.group_log2) : (kset / p.group));
         const uint32_t gs = 2 * grp, gz = (ZP ? 1 : 2) * grp;
 #pragma unroll
-        for (int f = 0; f < 2; ++f) {
+        for (int f = 0; f < NF; ++f) {
           const uint32_t a = ct + static_cast<uint32_t>(set * 4 * PR + r0 + 32 * f) * 4;
           const uint16_t s_lo = static_cast<uint16_t>(ld_shared_u32(a) >> (((cb[f][0] + gs) & 3) << 3));
           const uint16_t s_hi = static_cast<uint16_t>(ld_shared_u32(a + PR * 4) >> (((cb[f][1] + gs) & 3) << 3));
@@ -944,14 +954,14 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
         // steps 2 and 3 read set 1 with groups of 32, except in a K tail (K % 64 == 32) where their activations are zero
         // and set 0 stands in (no branch between the wgmma groups: set 0 is simply read again)
         const int set2 = (two_sets && kbase + 32 < p.K) ? 1 : 0;
-        typename D::Coef klo[2], khi[2];
+        typename D::Coef klo[NF], khi[NF];
         coefs(ct, 0, kbase, klo, khi);
-        uint32_t a[2][2][4];  // [step parity][fragment]: the registers of the step in flight stay untouched
+        uint32_t a[2][NF][4];  // [step parity][fragment]: the registers of the step in flight stay untouched
 #pragma unroll
         for (int st = 0; st < 4; ++st) {
           if (st == 2) coefs(ct, set2, kbase + 32 * set2, klo, khi);
 #pragma unroll
-          for (int f = 0; f < 2; ++f) {
+          for (int f = 0; f < NF; ++f) {
             uint32_t (&af)[4] = a[st & 1][f];
             fence_frag(af);
             const uint32_t chunk = wt + roff[f] + ((static_cast<uint32_t>(st) ^ rsw[f]) << 4);
@@ -965,17 +975,20 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
           wgmma_fence();
           const uint64_t db = wgmma_desc_sw128(act + st * 32);
 #pragma unroll
-          for (int f = 0; f < 2; ++f)
+          for (int f = 0; f < NF; ++f)
             wgmma_rs<Cfg::KIND, T>(*reinterpret_cast<float(*)[T / 2]>(acc + f * (T / 2)), a[st & 1][f], db,
                                    (st > 0 || accumulate) ? 1u : 0u);
-          // the last step is committed by consume_tile, whose wait retires step 2 before the next stage writes its set
+          // the last step is committed by consume_tile, whose wait retires step 2 before the next stage writes its set.
+          // One step in flight: with wait_group 2 (and four A buffers at T = 256) ptxas serialises the wgmmas (C7513).
           if (st < 3) {
             wgmma_commit();
             wgmma_wait<1>();  // retires step st - 1: its registers take step st + 1
           }
         }
       });
-      w4_epilogue<WT, T>(p, &tmap_out, acc, pipe.epi + wg * Cfg::EPI_TILE, m_blk * T, n_blk * PR + 64 * wg, wg);
+      // the staging tile of this warpgroup's packed rows (both warpgroups share one when NF = 1)
+      const int et = NF == 1 ? 0 : wg;
+      w4_epilogue<WT, T, NF>(p, &tmap_out, acc, pipe.epi + et * Cfg::EPI_TILE, m_blk * T, n_blk * PR + 64 * et, wg);
     }
     if ((threadIdx.x & 127) == 0) bulk_wait_group_all();  // the last tile's TMA store has completed
     if (p.g.n_out > 1) __threadfence_system();            // this thread's peer stores are performed before the rank signals

@@ -83,7 +83,7 @@ int make_tmap_2d_view(CUtensorMap* map, const void* base, int dt, int64_t rows, 
 
 // ---- test hooks (include/quanto_b200.h: qb200_test_override).  Every value selects a kernel that computes the same
 // result; 0 = automatic choice.  They exist so that the test-suite can execute every shipped instantiation.
-enum : int { OVR_TILE_M = 0 /* 64 | 128 rows per wgmma tile */, OVR_QBYTES_TILE_N = 1 /* int8: 128 | 256 */,
+enum : int { OVR_TILE_M = 0 /* 64 | 128 rows per wgmma tile; 256: the int4 swap-AB kernel at 256 tokens */, OVR_QBYTES_TILE_N = 1 /* int8: 128 | 256 */,
              OVR_INT4_ROUTE = 2, OVR_QBYTES_ROUTE = 3, OVR_GEMV_PRODUCER = 4,
              OVR_PDL = 5 /* 1 = no programmatic dependent launch */,
              OVR_GEMV_SHAPE = 6 /* 2 = the two-CTAs-per-SM shape of the ring gemv (M <= 2) */,

@@ -21,7 +21,9 @@ import torch
 SHAPES = [("gate_up_bf16", 4096, 14336, 4096, torch.bfloat16, False),
           ("down_bf16", 4096, 4096, 14336, torch.bfloat16, False),
           ("gate_up_f16_zp", 4096, 14336, 4096, torch.float16, True)] + \
-         [(f"m{m}_bf16", m, 14336, 4096, torch.bfloat16, False) for m in (32, 64, 128, 256, 512, 1024, 2048)]
+         [(f"m{m}_bf16", m, 14336, 4096, torch.bfloat16, False) for m in (32, 64, 128, 256, 300, 512, 1024, 2048)] + \
+         [(f"m{m}_n{n}_bf16", m, n, 4096, torch.bfloat16, False) for m, n in ((100, 128256), (128, 128256), (128, 33792),
+                                                                               (4097, 14336))]
 GROUP = 128
 DT = {torch.float16: 1, torch.bfloat16: 2}
 
