@@ -187,19 +187,62 @@ def ptr(t):
     return None if t is None else t.data_ptr()
 
 
-_workspaces = {}
+_workspaces = {}  # (device index, stream handle or _CAPTURE) -> zeroed uint8 buffer
+_outgrown = []  # buffers replaced by larger ones: never freed, a kernel in flight or a CUDA graph may still use them
+_CAPTURE = "capture"
+
+
+def _zeros_outside_graph_pools(index: int, nbytes: int) -> torch.Tensor:
+    """A zeroed buffer from the ordinary caching allocator, zeroed before this returns.
+
+    It is allocated on a helper thread: CUDA-graph warm-up (cudagraph trees) routes every allocation of the calling
+    thread into a graph's private pool, whose blocks a later graph may reuse.  Only ever called outside a capture.
+    """
+    result = []
+
+    def run():
+        try:
+            with torch.cuda.device(index):
+                buf = torch.zeros(nbytes, dtype=torch.uint8, device=f"cuda:{index}")
+                torch.cuda.current_stream(index).synchronize()
+            result.append(buf)
+        except BaseException as exc:  # handed to the calling thread
+            result.append(exc)
+
+    helper = threading.Thread(target=run, name="quanto-workspace")
+    helper.start()
+    helper.join()
+    if isinstance(result[0], BaseException):
+        raise result[0]
+    return result[0]
 
 
 def workspace(device, stream_handle: int, nbytes: int):
-    """Zero-initialised scratch for the stream-K small-M kernel, one per (device, stream); grown on demand.
+    """Zero-initialised scratch for the stream-K small-M kernel; grown on demand.
 
-    The kernel leaves the ticket counters zero on exit, so the buffer is zeroed only when (re)allocated.
+    The kernel leaves the ticket counters zero on exit, so a buffer is zeroed only when allocated.  Eager calls use one
+    buffer per (device, stream).  A call inside a CUDA-graph capture uses the device's capture buffer, which the eager
+    calls keep as large as the largest workspace they needed; a capture never allocates one.  Every buffer comes from the
+    ordinary allocator, never from a graph's pool, and is never freed, so the address a graph recorded stays valid and
+    is never handed to anything else.  Graphs replayed concurrently on different streams of one device would share the
+    capture buffer: replay them in order.
     """
     if nbytes <= 0:
         return None
-    key = (device.index if device.index is not None else torch.cuda.current_device(), stream_handle)
+    index = device.index if device.index is not None else torch.cuda.current_device()
+    capturing = torch.cuda.is_current_stream_capturing()
+    key = (index, _CAPTURE if capturing else stream_handle)
     ws = _workspaces.get(key)
-    if ws is None or ws.numel() < nbytes:
-        ws = torch.zeros(max(nbytes, 1 << 20), dtype=torch.uint8, device=device)
-        _workspaces[key] = ws
-    return ws
+    if ws is not None and ws.numel() >= nbytes:
+        return ws
+    if capturing:
+        raise NativeLibraryError(
+            f"quanto::qbits_mm: a CUDA-graph capture needs a {nbytes}-byte stream-K workspace that no call outside the "
+            "capture has prepared: run the captured code once before capturing it (a warm-up)")
+    for k in (key, (index, _CAPTURE)):
+        old = _workspaces.get(k)
+        if old is None or old.numel() < nbytes:
+            if old is not None:
+                _outgrown.append(old)
+            _workspaces[k] = _zeros_outside_graph_pools(index, max(nbytes, 1 << 20))
+    return _workspaces[key]

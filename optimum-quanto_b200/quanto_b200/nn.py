@@ -178,7 +178,9 @@ class QModuleMixin:
     def quantize_input(self, module, input):
         input = input[0]
         if isinstance(input, ActivationQBytesTensor):
-            if input.qtype != self.activation_qtype:
+            # compared by storage dtype (one per 8-bit qtype): under torch.compile an activation created inside the
+            # graph exposes only tensors and literals, not its qtype object
+            if input._data.dtype != self.activation_qtype.dtype:
                 raise ValueError(
                     "Models with heterogeneous quantized activations are not supported:"
                     f" expected {self.activation_qtype.name} input but got {input.qtype.name} instead."
@@ -187,7 +189,7 @@ class QModuleMixin:
         return quantize_activation(input, qtype=self.activation_qtype, scale=self.input_scale)
 
     def quantize_output(self, module, input, output):
-        if isinstance(output, ActivationQBytesTensor) and output.qtype == self.activation_qtype:
+        if isinstance(output, ActivationQBytesTensor) and output._data.dtype == self.activation_qtype.dtype:
             return output  # QLinear.forward already quantised it in the GEMM epilogue (one launch, see below)
         return quantize_activation(output, qtype=self.activation_qtype, scale=self.output_scale)
 
@@ -223,7 +225,7 @@ class QLinear(QModuleMixin, torch.nn.Linear):
         w = self.weight
         if ("output" not in self._quantize_hooks or not isinstance(input, ActivationQBytesTensor)
                 or not isinstance(w, WeightQBytesTensor) or not w._data.is_cuda or w.axis != 0 or w.ndim != 2
-                or input.qtype != self.activation_qtype
+                or input._data.dtype != self.activation_qtype.dtype
                 or (torch.is_grad_enabled() and (input.requires_grad or w.requires_grad))):
             return None
         scales = input._scale * w._scale  # in the module dtype, one rounding (tensor/weights/qbytes.py:72-73)

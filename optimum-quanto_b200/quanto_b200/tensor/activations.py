@@ -51,10 +51,13 @@ class ActivationQBytesTensor(QBytesTensor):
     @staticmethod
     def __tensor_unflatten__(inner_tensors, meta, outer_size, outer_stride):
         assert len(inner_tensors) == 2 and len(meta) == 3
+        # under tracing the outer size may be symbolic (a dynamic token count): it is passed in, not parsed from meta
+        size = ast.literal_eval(meta["size"]) if outer_size is None else outer_size
+        stride = ast.literal_eval(meta["stride"]) if outer_stride is None else outer_stride
         return ActivationQBytesTensor(
             qtypes[meta["qtype"]],
-            ast.literal_eval(meta["size"]),
-            ast.literal_eval(meta["stride"]),
+            size,
+            stride,
             inner_tensors["_data"],
             inner_tensors["_scale"],
         )

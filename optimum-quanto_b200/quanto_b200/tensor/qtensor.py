@@ -94,7 +94,7 @@ class QBytesTensor(QTensor):
         return f"{type(self).__name__}({self._data}, scale={self._scale}, dtype={self.dtype})"
 
     def _dequantize_impl(self):
-        payload = self._data.to(self._scale.dtype) if self.qtype.is_floating_point else self._data  # fp8 has no mul
+        payload = self._data.to(self._scale.dtype) if self._data.dtype.is_floating_point else self._data  # fp8: no mul
         return self._scale * payload
 
     def dequantize(self):
