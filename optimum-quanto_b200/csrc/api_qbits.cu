@@ -129,6 +129,7 @@ static int qbits_mm_impl(QbitsArgs& q) {
   p.group = group;
   p.group_log2 = q.group_log2;
   p.shift_is_int = q.shift_is_int;
+  p.dbg = debug_flags();
   const int tile_m = wgmma_tile_m(m);
   const int64_t half_n = n / 2;
   // OVR_TILE_M = 256 names the swap-AB kernel's 256-token tile, at any shape

@@ -66,6 +66,7 @@ struct GemmParams {
   // BSrc::INT4: 1 = the epilogue stores each tile with TMA through `tmap_out` (one dense [M, N] output: g.n_out = 1,
   // ld = N, col0 = 0, N % 16 == 0); 0 = ordinary stores
   int epi_tma;
+  int dbg;  // developer knock-outs (debug_flags(); always 0 in the release library, see QB_KO)
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -952,25 +953,31 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
         const uint32_t act = wt - Cfg::A_TILE, ct = wt + Cfg::W_TILE;
         const int kbase = 64 * kb++;
         // steps 2 and 3 read set 1 with groups of 32, except in a K tail (K % 64 == 32) where their activations are zero
-        // and set 0 stands in (no branch between the wgmma groups: set 0 is simply read again)
-        const int set2 = (two_sets && kbase + 32 < p.K) ? 1 : 0;
+        // and set 0 stands in.  Otherwise the stage has one set and steps 2 and 3 keep the coefficients of step 0:
+        // re-reading them put four shared loads and the coefficient arithmetic in front of step 2's wgmma (the branch is
+        // uniform over the warpgroup, and ptxas keeps the wgmmas asynchronous).
+        const bool set2 = two_sets && kbase + 32 < p.K;
         typename D::Coef klo[NF], khi[NF];
         coefs(ct, 0, kbase, klo, khi);
         uint32_t a[2][NF][4];  // [step parity][fragment]: the registers of the step in flight stay untouched
 #pragma unroll
         for (int st = 0; st < 4; ++st) {
-          if (st == 2) coefs(ct, set2, kbase + 32 * set2, klo, khi);
+          if (st == 2 && set2) coefs(ct, 1, kbase + 32, klo, khi);
 #pragma unroll
           for (int f = 0; f < NF; ++f) {
             uint32_t (&af)[4] = a[st & 1][f];
             fence_frag(af);
             const uint32_t chunk = wt + roff[f] + ((static_cast<uint32_t>(st) ^ rsw[f]) << 4);
             const uint32_t x = __byte_perm(ld_shared_u32(chunk), ld_shared_u32(chunk + 8), sel);
-            const uint32_t wl = x & 0x0F0F0F0Fu, wh = (x >> 4) & 0x0F0F0F0Fu;
-            af[0] = D::cvt(__byte_perm(wl, D::MAGIC_BYTES, 0x4140), klo[f], ZP);  // row g,     k 2c, 2c+1
-            af[1] = D::cvt(__byte_perm(wh, D::MAGIC_BYTES, 0x4140), khi[f], ZP);  // row g + 8, k 2c, 2c+1
-            af[2] = D::cvt(__byte_perm(wl, D::MAGIC_BYTES, 0x4342), klo[f], ZP);  // row g,     k 2c+8, 2c+9
-            af[3] = D::cvt(__byte_perm(wh, D::MAGIC_BYTES, 0x4342), khi[f], ZP);  // row g + 8, k 2c+8, 2c+9
+            if (QB_KO(p.dbg, 1)) {  // developer experiment: no dequantisation, the raw packed word as the A fragment
+              af[0] = af[1] = af[2] = af[3] = x;
+            } else {
+              const uint32_t wl = x & 0x0F0F0F0Fu, wh = (x >> 4) & 0x0F0F0F0Fu;
+              af[0] = D::cvt(__byte_perm(wl, D::MAGIC_BYTES, 0x4140), klo[f], ZP);  // row g,     k 2c, 2c+1
+              af[1] = D::cvt(__byte_perm(wh, D::MAGIC_BYTES, 0x4140), khi[f], ZP);  // row g + 8, k 2c, 2c+1
+              af[2] = D::cvt(__byte_perm(wl, D::MAGIC_BYTES, 0x4342), klo[f], ZP);  // row g,     k 2c+8, 2c+9
+              af[3] = D::cvt(__byte_perm(wh, D::MAGIC_BYTES, 0x4342), khi[f], ZP);  // row g + 8, k 2c+8, 2c+9
+            }
           }
           wgmma_fence();
           const uint64_t db = wgmma_desc_sw128(act + st * 32);
@@ -997,9 +1004,14 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
     if (warp == L::PRODUCER_WARP && lane == 0) {
       // ---------------------------------------------------------------- TMA producer: activations + packed bytes
       gather_wait_start(p.g);  // the activation may be the gathered output of the previous linear
-      pipe.produce(num_tiles, p.num_m_blocks, kblocks, Cfg::A_TILE + Cfg::W_TILE,
+      // developer experiment 8: no activation feed after the first NSTAGES k-blocks of a tile (the stages keep stale data)
+      const bool no_act = QB_KO(p.dbg, 8);
+      pipe.produce(num_tiles, p.num_m_blocks, kblocks, (no_act ? 0 : Cfg::A_TILE) + Cfg::W_TILE,
                    [&](uint8_t* dst, uint64_t* bar, int m_blk, int n_blk, int kb) {
-                     tma_load_2d(dst, &tmap_a, bar, kb * 64, m_blk * T);
+                     if (!no_act || kb < L::NSTAGES) {
+                       if (no_act) mbar_expect_tx(bar, Cfg::A_TILE);
+                       tma_load_2d(dst, &tmap_a, bar, kb * 64, m_blk * T);
+                     }
                      tma_load_2d(dst + Cfg::A_TILE, &tmap_w, bar, kb * 64, n_blk * PR);
                    });
     } else if (warp == L::PRODUCER_WARP + 1) {
@@ -1019,7 +1031,7 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
             const int row = e - set * PR;
             const int rp = n_blk * PR + row;
             // rows past N/2 are never stored; a K-tail second group (K % 64 == 32) is never read
-            if (rp >= half_n || (set == 1 && kbase + 32 >= p.K)) continue;
+            if (rp >= half_n || (set == 1 && kbase + 32 >= p.K) || QB_KO(p.dbg, 4)) continue;
             const size_t ilo = static_cast<size_t>(rp) * gpr + g0 + set;
             const size_t ihi = ilo + static_cast<size_t>(half_n) * gpr;
             const uint32_t d = ct + static_cast<uint32_t>(set * 4 * PR + row) * 4;
