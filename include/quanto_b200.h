@@ -150,6 +150,40 @@ QB200_API int qb200_qbytes_mm_quantized(const void* a, const void* w, const void
                                         const void* out_scale, int64_t m, int64_t n, int64_t k, int a_dtype, int w_dtype,
                                         int scale_dtype, int q_dtype, void* stream);
 
+/* ---- quantized attention: per-tensor int8 / float8 activations kept quantized (the reference's ActivationQBytesTensor
+ * op table, optimum/quanto/tensor/activations/qbytes_ops.py) ------------------------------------------------------ */
+
+/* aten.bmm of two qint8 activations (qbytes_ops.py:175-186):
+ *   out[b] = rnd_dt( f32(A[b] @ B[b]) * f32(rnd_dt(scale_a * scale_b)) )
+ * with the sum an exact int32 sum (bit-identical to the reference's fp32 bmm whenever K <= 1024).
+ * A: int8 [batch, m, k], rows dense, batch b at a + b * a_batch_stride (0 = one A for every batch).
+ * B: int8, element (k, n) of batch b at b + b * b_batch_stride + (b_layout == 0 ? n * k + k : k * n + n): layout 0 is
+ * K-contiguous (a transposed key), layout 1 N-contiguous (a value, or a key after matmul's reshape); stride 0 = one B
+ * for every batch (an expanded operand, read in place).
+ * scale_a, scale_b: ONE element each (device memory) of scale_dtype in {F32, F16, BF16}; out: dense [batch, m, n] of
+ * scale_dtype.
+ * K % 16 == 0 with A 16-byte aligned runs on the tensor cores (wgmma, family 1); an N-contiguous B is first copied
+ * K-major by one byte-transpose pass into `workspace` (family 4), which must hold
+ * qb200_qbytes_bmm_workspace_bytes(...) bytes, 16-byte aligned, owned by the call until the stream reaches its end.
+ * Every other problem runs on a CUDA-core kernel with the same exact sum and roundings (family 2). */
+QB200_API int qb200_qbytes_bmm(const void* a, const void* b, const void* scale_a, const void* scale_b, void* out,
+                               void* workspace, int64_t workspace_bytes, int64_t batch, int64_t m, int64_t n, int64_t k,
+                               int64_t a_batch_stride, int64_t b_batch_stride, int b_layout, int scale_dtype,
+                               void* stream);
+
+/* Bytes of workspace qb200_qbytes_bmm needs for this B (0 when B is read in place). */
+QB200_API int64_t qb200_qbytes_bmm_workspace_bytes(int64_t batch, int64_t n, int64_t k, int64_t b_batch_stride,
+                                                   int b_layout);
+
+/* aten._softmax over the last dim of a per-tensor quantized activation, re-quantized (qbytes_ops.py:208-215), in one
+ * launch: x, out: [rows, cols] codes of q_dtype in {I8, E4M3, E5M2, E4M3FNUZ}; scale (the input's) and out_scale
+ * (1 / qmax rounded to the scale dtype, as torch.tensor(1 / qmax, dtype=...) gives it): ONE element each of
+ * scale_dtype in {F32, F16, BF16}, device memory.  Per row: x = rnd_dt(scale * payload), y = rnd_dt(softmax(x)) with
+ * fp32 max / exp / sum, out = quantize_symmetric(y, q_dtype, out_scale).  Any row length; rows of up to 32768 codes are
+ * read from memory once. */
+QB200_API int qb200_qbytes_softmax(const void* x, const void* scale, const void* out_scale, void* out, int64_t rows,
+                                   int64_t cols, int q_dtype, int scale_dtype, void* stream);
+
 /* ---- input gradient of the quantized linear (the backward's dX = gO @ W) ---------------------------------------- */
 
 /* grad_in[M, K] = grad_out[M, N] @ dequant(packed, scale, shift)[N, K] in one launch, reading the packed weights.
@@ -238,8 +272,9 @@ QB200_API int64_t qb200_quantize_qbits_hqq_workspace_bytes(int64_t n, int64_t k,
 QB200_API int qb200_hqq_shrink(const void* x, void* out, int64_t numel, double beta, double lp_norm, int dtype,
                                void* stream);
 
-/* Which kernel family the last qb200_qbytes_mm / qb200_qbits_mm / *_grad_input call on this thread dispatched to:
- * 0 none, 1 wgmma (TMA + warpgroup MMA), 2 CUDA-core (shape-agnostic), 3 warp-MMA gemv (int4, M <= 32: TMA ring or register streaming).
+/* Which kernel family the last qb200_qbytes_mm / qb200_qbytes_bmm / qb200_qbits_mm / *_grad_input call on this thread dispatched to:
+ * 0 none, 1 wgmma (TMA + warpgroup MMA), 2 CUDA-core (shape-agnostic), 3 warp-MMA gemv (int4, M <= 32: TMA ring or register streaming),
+ * 4 byte-transpose pass + wgmma (qb200_qbytes_bmm with a B that is not K-contiguous).
  * For tests and bench accounting. */
 QB200_API int qb200_last_kernel_family(void);
 
@@ -254,7 +289,9 @@ QB200_API int qb200_last_kernel_family(void);
  *   key 5  programmatic dependent launch   : 1 off
  *   key 6  ring-gemv shape (M <= 2)        : 2 two CTAs per SM (opt-in experiment; default one CTA per SM)
  *   key 7  int4 wgmma epilogue             : 1 ordinary stores (default: TMA stores from a shared-memory tile when the
- *                                            output is one dense [M, N] buffer with N % 16 == 0) */
+ *                                            output is one dense [M, N] buffer with N % 16 == 0)
+ *   key 8  qbytes_bmm route                : 2 CUDA-core kernel, 3 byte-transpose pass + wgmma for either B layout
+ *                                            (default: wgmma reading a K-contiguous B in place) */
 QB200_API int qb200_test_override(int key, int value);
 
 /* Developer aids.  They act only in a library built with `make KNOCKOUTS=1` (qb200_developer_build() == 1); in the

@@ -178,6 +178,25 @@ int make_tmap_packed(CUtensorMap* map, const uint8_t* packed, int64_t rows, int6
   return encode_2d(map, packed, DT_U8, rows, cols, cols, 64, box_rows, CU_TENSOR_MAP_SWIZZLE_64B);
 }
 
+int make_tmap_3d_bytes(CUtensorMap* map, const void* base, int64_t batch, int64_t rows, int64_t cols,
+                       int64_t batch_stride, int box_rows) {
+  EncodeTiledFn enc = get_encode_fn();
+  if (enc == nullptr) return fail(ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
+  if (reinterpret_cast<uintptr_t>(base) % 16 != 0) return fail(ERR_ARG, "TMA operand not 16-byte aligned");
+  if (cols % 16 != 0 || batch_stride % 16 != 0)
+    return fail(ERR_ARG, "TMA row pitch %lld / batch stride %lld not a multiple of 16 bytes", (long long)cols,
+                (long long)batch_stride);
+  const cuuint64_t gdim[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows), static_cast<cuuint64_t>(batch)};
+  const cuuint64_t gstride[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(batch_stride)};
+  const cuuint32_t box[3] = {128, static_cast<cuuint32_t>(box_rows), 1};
+  const cuuint32_t estride[3] = {1, 1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(base), gdim, gstride, box, estride,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(ERR_CUDA, "cuTensorMapEncodeTiled (3-d) failed with CUresult %d", static_cast<int>(r));
+  return OK;
+}
+
 int make_tmap_2d_view(CUtensorMap* map, const void* base, int dt, int64_t rows, int64_t cols, int64_t pitch_elems,
                       int box_cols, int box_rows, bool swizzle128) {
   return encode_2d(map, base, dt, rows, cols, pitch_elems, box_cols, box_rows,

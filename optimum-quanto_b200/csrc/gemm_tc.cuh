@@ -67,6 +67,14 @@ struct GemmParams {
   // ld = N, col0 = 0, N % 16 == 0); 0 = ordinary stores
   int epi_tma;
   int dbg;  // developer knock-outs (debug_flags(); always 0 in the release library, see QB_KO)
+  // Batched int8 x int8 (GemmCfg::BATCH, quanto::qbytes_bmm): out[b] = A[b] @ B[b]^T, with rank-3 tensor maps
+  // [batch, rows, K] for both operands.  num_n_blocks = batch * n_blocks_per_batch (tile t: m-block t % num_m_blocks,
+  // then n-block, then batch); `out` is the dense [batch, M, N] output.  The output scale is the ONE scalar
+  // rnd_out(scales[0] * scale_b[0]) (the two per-tensor activation scales).  a_batch_mul / b_batch_mul are 0 for an
+  // operand broadcast over the batch (its tensor map has one batch), else 1.
+  const void* scale_b;
+  int n_blocks_per_batch;
+  int a_batch_mul, b_batch_mul;
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -307,11 +315,13 @@ __device__ __forceinline__ void stage_row_64k(const uint4 (&raw)[4], uint32_t s2
 // ------------------------------------------------------------------------------------------------
 // KIND_: MMA operand kind (F16 / BF16, or I8 for int8 x int8).  MWG_: consumer warpgroups (BM = 64 * MWG_).
 // WT_: staged element type (INT4 / BYTES / F8).
+// BATCH_: the batched int8 x int8 product of quanto::qbytes_bmm (see GemmParams).
 template <MmaKind KIND_, BSrc BSRC_, int MWG_, int BN_, typename WT_ = __nv_bfloat16, bool ZP_ = false, int WKIND_ = 0,
-          int AKIND_ = 0>
+          int AKIND_ = 0, bool BATCH_ = false>
 struct GemmCfg {
   static constexpr MmaKind KIND = KIND_;
   static constexpr BSrc BSRC = BSRC_;
+  static constexpr bool BATCH = BATCH_;
   static constexpr bool ZP = ZP_;       // INT4 only: shift is an integer zero-point (compile-time: keeps the hot loop lean)
   static constexpr int WKIND = WKIND_;  // BYTES / F8: weight bytes: 0 int8, 1 float8_e4m3fn, 2 float8_e5m2, 3 float8_e4m3fnuz
   static constexpr int AKIND = AKIND_;  // F8: activation bytes, same codes
@@ -335,6 +345,7 @@ struct GemmCfg {
                           MWG * EPI_TILE>;
   static_assert(BN == 128 || (BN == 256 && IS_INT && BSRC == BSrc::TMA), "wgmma tile width");
   static_assert(BSRC == BSrc::TMA || KIND == MmaKind::F16 || KIND == MmaKind::BF16, "staged weights are 16-bit");
+  static_assert(!BATCH || (IS_INT && BSRC == BSrc::TMA), "batched: int8 x int8 with both operands fed by TMA");
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -361,9 +372,10 @@ __device__ __forceinline__ void store_pair(OT* dst, float a, float b, bool two, 
 }
 
 // f0, f1: accumulator values of output features n, n + 1 (n + 1 only when `two`); row_off = row * ld + col0.
-template <typename OT, bool ALLOW_Q>
+// PER_N = false: the caller has applied the scale already (the batched kernel's one scalar), p.scales is not read.
+template <typename OT, bool ALLOW_Q, bool PER_N = true>
 __device__ __forceinline__ void epilogue_pair_t(const GemmParams& p, size_t row_off, int n, bool two, float f0, float f1) {
-  if (p.scales != nullptr) {
+  if (PER_N && p.scales != nullptr) {
     f0 = __fmul_rn(f0, load_out_dt_as_float(p.scales, p.out_dt, n));
     if (two) f1 = __fmul_rn(f1, load_out_dt_as_float(p.scales, p.out_dt, n + 1));
   }
@@ -401,11 +413,20 @@ __device__ __forceinline__ void epilogue_pair_t(const GemmParams& p, size_t row_
   for (int q = 0; q < p.g.n_out; ++q) store_pair<OT>(static_cast<OT*>(p.g.out_peer[q]) + row_off + n, f0, f1, two, vec);
 }
 
-template <bool ALLOW_Q>
+template <bool ALLOW_Q, bool PER_N = true>
 __device__ __forceinline__ void epilogue_pair(const GemmParams& p, size_t row_off, int n, bool two, float f0, float f1) {
-  if (p.out_dt == DT_BF16) epilogue_pair_t<__nv_bfloat16, ALLOW_Q>(p, row_off, n, two, f0, f1);
-  else if (p.out_dt == DT_F16) epilogue_pair_t<__half, ALLOW_Q>(p, row_off, n, two, f0, f1);
-  else epilogue_pair_t<float, ALLOW_Q>(p, row_off, n, two, f0, f1);
+  if (p.out_dt == DT_BF16) epilogue_pair_t<__nv_bfloat16, ALLOW_Q, PER_N>(p, row_off, n, two, f0, f1);
+  else if (p.out_dt == DT_F16) epilogue_pair_t<__half, ALLOW_Q, PER_N>(p, row_off, n, two, f0, f1);
+  else epilogue_pair_t<float, ALLOW_Q, PER_N>(p, row_off, n, two, f0, f1);
+}
+
+// rnd_dt(sa * sb) of two one-element scales of dtype `dt`: the output scale of the reference's int8 bmm
+// (tensor/activations/qbytes_ops.py:185, `input._scale * other._scale` in the scale dtype, then widened to fp32).
+__device__ __forceinline__ float scalar_scale_product(const void* sa, const void* sb, int dt) {
+  const float s = __fmul_rn(load_out_dt_as_float(sa, dt, 0), load_out_dt_as_float(sb, dt, 0));
+  if (dt == DT_BF16) return rnd<__nv_bfloat16>(s);
+  if (dt == DT_F16) return rnd<__half>(s);
+  return s;
 }
 
 // Epilogue of the int4 kernels (output dtype OT = the 16-bit activation dtype), one consumer warpgroup's 64-row slice
@@ -522,9 +543,17 @@ __global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
     using AccT = typename std::conditional<Cfg::IS_INT, uint32_t, float>::type;
     AccT acc[Cfg::NACC];
     RingPos<L::NSTAGES> pos;
+    float s_ab = 0.f;
+    if constexpr (Cfg::BATCH) s_ab = scalar_scale_product(p.scales, p.scale_b, p.out_dt);
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m_blk = tile % p.num_m_blocks;
-      const int n_blk = tile / p.num_m_blocks;
+      int n_blk = tile / p.num_m_blocks;
+      size_t out_base = 0;  // first element of the tile's batch in the output
+      if constexpr (Cfg::BATCH) {
+        const int b = n_blk / p.n_blocks_per_batch;
+        n_blk -= b * p.n_blocks_per_batch;
+        out_base = static_cast<size_t>(b) * p.M * p.ld;
+      }
       pipe.consume_tile(pos, kblocks, acc, [&](uint32_t aa, uint32_t bb, bool accumulate) {
         wgmma_slab<Cfg::KIND, BN>(acc, aa, bb, accumulate);
       });
@@ -538,7 +567,7 @@ __global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
         for (int h = 0; h < 2; ++h) {
           const int row = r0 + 8 * h;
           if (row >= p.M) continue;
-          const size_t row_off = static_cast<size_t>(row) * p.ld + p.col0;
+          const size_t row_off = out_base + static_cast<size_t>(row) * p.ld + p.col0;
 #pragma unroll
           for (int j = 0; j < BN / 8; ++j) {
             const int n = n_blk * BN + 8 * j + 2 * (lane & 3);
@@ -551,7 +580,13 @@ __global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
               f0 = acc[4 * j + 2 * h];
               f1 = acc[4 * j + 2 * h + 1];
             }
-            epilogue_pair<Cfg::BSRC == BSrc::TMA || Cfg::BSRC == BSrc::F8>(p, row_off, n, n + 1 < p.N, f0, f1);
+            if constexpr (Cfg::BATCH) {
+              f0 = __fmul_rn(f0, s_ab);
+              f1 = __fmul_rn(f1, s_ab);
+              epilogue_pair<false, false>(p, row_off, n, n + 1 < p.N, f0, f1);
+            } else {
+              epilogue_pair<Cfg::BSRC == BSrc::TMA || Cfg::BSRC == BSrc::F8>(p, row_off, n, n + 1 < p.N, f0, f1);
+            }
           }
         }
       }
@@ -565,8 +600,15 @@ __global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
       constexpr uint32_t tx_bytes = Cfg::A_TILE + (Cfg::BSRC == BSrc::TMA ? Cfg::B_TILE : 0);
       gather_wait_start(p.g);  // the activation may be the gathered output of the previous linear
       pipe.produce(num_tiles, p.num_m_blocks, kblocks, tx_bytes, [&](uint8_t* dst, uint64_t* bar, int m_blk, int n_blk, int kb) {
-        tma_load_2d(dst, &tmap_a, bar, kb * KELEMS, m_blk * Cfg::BM);
-        if constexpr (Cfg::BSRC == BSrc::TMA) tma_load_2d(dst + Cfg::A_TILE, &tmap_b, bar, kb * KELEMS, n_blk * BN);
+        if constexpr (Cfg::BATCH) {
+          const int b = n_blk / p.n_blocks_per_batch;
+          tma_load_3d(dst, &tmap_a, bar, kb * KELEMS, m_blk * Cfg::BM, b * p.a_batch_mul);
+          tma_load_3d(dst + Cfg::A_TILE, &tmap_b, bar, kb * KELEMS, (n_blk - b * p.n_blocks_per_batch) * BN,
+                      b * p.b_batch_mul);
+        } else {
+          tma_load_2d(dst, &tmap_a, bar, kb * KELEMS, m_blk * Cfg::BM);
+          if constexpr (Cfg::BSRC == BSrc::TMA) tma_load_2d(dst + Cfg::A_TILE, &tmap_b, bar, kb * KELEMS, n_blk * BN);
+        }
       });
     }
   } else if constexpr (Cfg::BSRC == BSrc::INT4) {

@@ -77,6 +77,10 @@ int make_tmap_planes(CUtensorMap* map, const void* base, int dt, int64_t rows, i
 // Packed int4 weights [rows, cols] bytes; box = 64 bytes of a row x box_rows rows, 64-byte swizzle (16-byte chunk s of
 // row r at chunk s ^ ((r >> 1) & 3)).
 int make_tmap_packed(CUtensorMap* map, const uint8_t* packed, int64_t rows, int64_t cols, int box_rows);
+// [batch, rows, cols] bytes, rows dense (pitch = cols), batches `batch_stride` bytes apart; box = 128 bytes of a row x
+// box_rows rows of one batch, 128-byte swizzle.  A box never crosses a batch: past `rows` TMA fills zeros.
+int make_tmap_3d_bytes(CUtensorMap* map, const void* base, int64_t batch, int64_t rows, int64_t cols,
+                       int64_t batch_stride, int box_rows);
 // [rows, cols] view with an explicit row pitch and box: the epilogue's TMA stores into (a column slab of) the output.
 int make_tmap_2d_view(CUtensorMap* map, const void* base, int dt, int64_t rows, int64_t cols, int64_t pitch_elems,
                       int box_cols, int box_rows, bool swizzle128);
@@ -87,11 +91,15 @@ enum : int { OVR_TILE_M = 0 /* 64 | 128 rows per wgmma tile; 256: the int4 swap-
              OVR_INT4_ROUTE = 2, OVR_QBYTES_ROUTE = 3, OVR_GEMV_PRODUCER = 4,
              OVR_PDL = 5 /* 1 = no programmatic dependent launch */,
              OVR_GEMV_SHAPE = 6 /* 2 = the two-CTAs-per-SM shape of the ring gemv (M <= 2) */,
-             OVR_INT4_EPILOGUE = 7 /* 1 = the int4 wgmma epilogue stores without TMA */, OVR_COUNT = 8 };
+             OVR_INT4_EPILOGUE = 7 /* 1 = the int4 wgmma epilogue stores without TMA */,
+             OVR_BMM_ROUTE = 8 /* qbytes_bmm: 2 = CUDA-core kernel, 3 = K-major copy of B + wgmma for any B layout */,
+             OVR_COUNT = 9 };
 // OVR_INT4_ROUTE values
 enum : int { ROUTE_AUTO = 0, ROUTE_INT4_GENERAL = 1, ROUTE_INT4_GEMV = 3, ROUTE_INT4_RING = 4, ROUTE_INT4_RING2 = 8 };
 // OVR_QBYTES_ROUTE values
 enum : int { ROUTE_QBYTES_SIMT = 2 };
+// OVR_BMM_ROUTE values
+enum : int { ROUTE_BMM_SIMT = 2, ROUTE_BMM_TRANSPOSE = 3 };
 int test_override(int key);
 
 // Rows per wgmma tile: one consumer warpgroup (64 rows) while M <= 64, so that small batches do not pay for empty MMA

@@ -5,6 +5,7 @@ mirror of the reference classes on the hot path.  The native library is loaded l
 its absence is an error (no CPU / eager fallback).
 """
 from . import library  # noqa: F401  (op registration side effect)
+from . import library_attention  # noqa: F401  (quantized attention ops)
 from .calibrate import *  # noqa: F401,F403
 from .nn import *  # noqa: F401,F403
 from .pipeline import *  # noqa: F401,F403

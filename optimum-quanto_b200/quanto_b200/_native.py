@@ -58,13 +58,17 @@ EXPORTS = (
     "qb200_quantize_qbits_hqq",
     "qb200_quantize_qbits_hqq_workspace_bytes",
     "qb200_hqq_shrink",
+    "qb200_qbytes_bmm",
+    "qb200_qbytes_bmm_workspace_bytes",
+    "qb200_qbytes_softmax",
 )
 
 # qb200_test_override keys (include/quanto_b200.h)
 (OVR_TILE_M, OVR_QBYTES_TILE_N, OVR_INT4_ROUTE, OVR_QBYTES_ROUTE, OVR_GEMV_PRODUCER, OVR_PDL, OVR_GEMV_SHAPE,
- OVR_INT4_EPILOGUE) = range(8)
+ OVR_INT4_EPILOGUE, OVR_BMM_ROUTE) = range(9)
 ROUTE_INT4_GENERAL, ROUTE_INT4_GEMV, ROUTE_INT4_RING, ROUTE_INT4_RING2 = 1, 3, 4, 8
 ROUTE_QBYTES_SIMT = 2
+ROUTE_BMM_SIMT, ROUTE_BMM_TRANSPOSE = 2, 3
 GATHER_WAIT_INPUT, GATHER_WAIT_OUTPUT = 1, 2
 
 
@@ -144,6 +148,10 @@ def load():
         lib.qb200_quantize_qbits_hqq_workspace_bytes.argtypes = [i64, i64, i32, i32]
         lib.qb200_quantize_qbits_hqq_workspace_bytes.restype = i64
         lib.qb200_hqq_shrink.argtypes = [vp, vp, i64, f64, f64, i32, vp]
+        lib.qb200_qbytes_bmm.argtypes = [vp, vp, vp, vp, vp, vp, i64, i64, i64, i64, i64, i64, i64, i32, i32, vp]
+        lib.qb200_qbytes_bmm_workspace_bytes.argtypes = [i64, i64, i64, i64, i32]
+        lib.qb200_qbytes_bmm_workspace_bytes.restype = i64
+        lib.qb200_qbytes_softmax.argtypes = [vp, vp, vp, vp, i64, i64, i32, i32, vp]
         for name in EXPORTS:
             getattr(lib, name)  # AttributeError here == header and library out of sync
         # Developer knock-outs exist only in a `make KNOCKOUTS=1` build and are set explicitly through

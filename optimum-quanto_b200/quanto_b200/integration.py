@@ -22,12 +22,17 @@ After this, every `optimum.quanto` object keeps working as before -- `quantize()
 4. `WeightQBytesLinearFunction.forward` (tensor/weights/qbytes.py:68-82) keeps calling `quanto::qbytes_mm`, with the bias
    fused into the kernel epilogue when there is one; its backward takes the input gradient from
    `quanto::qbytes_grad_input` the same way;
+6. `aten.bmm` and `aten._softmax` of the reference's `ActivationQBytesTensor` table
+   (tensor/activations/qbytes_ops.py:175-186, 208-215) run on `quanto::qbytes_bmm` (an exact int8 x int8 product on the
+   tensor cores instead of an fp32 bmm of int8 values cast to fp32) and `quanto::qbytes_softmax` (codes in, codes out,
+   one launch) for CUDA tensors; every case those entries decline falls through to the reference's own entry.
 5. `HqqOptimizer.__call__` (tensor/optimizers/hqq_optimizer.py:60-87 after affine_optimizer.py:27-64) runs
    `quanto::quantize_qbits_hqq` -- two launches, no host synchronisation -- for a CUDA bf16 / fp16 weight quantized along
    axis 0 to qint4 / qint2, and the reference's own code for everything else and whatever the kernel declines.
 
 Used by tools/run_reference_tests.py to run the reference's OWN hot-path tests (tests/library, tests/tensor/ops,
-tests/nn/test_qlinear.py) against these kernels.  Nothing here is imported by the rest of the package.
+tests/nn/test_qlinear.py, and for 6 tests/tensor/ops/test_mm_dispatch.py, tests/tensor/activations/test_activations_dispatch.py,
+tests/nn/test_qattention.py) against these kernels.  Nothing here is imported by the rest of the package.
 """
 import torch
 
@@ -154,4 +159,36 @@ def bind_reference():
         return orig_hqq_call(self, base, qtype, axis, group_size, zeropoint)
 
     RefHqq.__call__ = hqq_call
+
+    # ---- 6. quantized attention: int8 bmm and softmax of per-tensor activations
+    from optimum.quanto.tensor.activations import qbytes_ops as ref_ops
+    from optimum.quanto.tensor.activations.qbytes import ActivationQBytesTensor as RefActivation
+    from optimum.quanto.tensor.core import dtype_info as ref_dtype_info
+    from optimum.quanto.tensor.qtype import qint8 as ref_qint8
+
+    from . import library_attention  # noqa: F401  (defines quanto::qbytes_bmm / quanto::qbytes_softmax)
+
+    aten = torch.ops.aten
+    table = ref_ops._QBYTESTENSOR_OP_TABLE
+    orig_bmm, orig_softmax = table[aten.bmm], table[aten._softmax]
+
+    def per_tensor(t):
+        return isinstance(t, RefActivation) and t.axis is None and t._data.is_cuda and t._scale.numel() == 1
+
+    def bmm(input, other):
+        if (per_tensor(input) and per_tensor(other) and input.qtype == ref_qint8 and other.qtype == ref_qint8
+                and other._scale.dtype == input._scale.dtype):
+            return torch.ops.quanto.qbytes_bmm(input._data, other._data, input._scale, other._scale)
+        return orig_bmm(input, other)
+
+    def softmax(input, dim, half_to_float):
+        if per_tensor(input) and not half_to_float and dim in (-1, input.ndim - 1):
+            out_scale = torch.tensor(1 / ref_dtype_info(input.qtype.dtype).max, dtype=input._scale.dtype).to(
+                input.device)
+            data = torch.ops.quanto.qbytes_softmax(input._data, input._scale, out_scale)
+            return RefActivation(input.qtype, data.size(), data.stride(), data, out_scale)
+        return orig_softmax(input, dim, half_to_float)
+
+    table[aten.bmm] = bmm
+    table[aten._softmax] = softmax
     _bound = True

@@ -1,9 +1,9 @@
 """Per-tensor 8-bit quantized activations (optimum/quanto/tensor/activations/qbytes.py:28-92, quantization.py:24-39).
 
-Only what the linear hot path needs is kept: construction through `quanto::quantize_symmetric` (one sm_90a kernel),
-flatten/unflatten, and a dequantising fallback for every aten op.  The reference's table of quantized attention ops
-(qbytes_ops.py) is out of scope (SURVEY 2, row 14); `F.linear` never reaches it because the weight's
-`__torch_function__` intercepts first.
+Construction through `quanto::quantize_symmetric` (one sm_90a kernel), flatten/unflatten, and the reference's aten op
+table (qbytes_ops.py, ported in activation_ops.py): layout ops keep the tensor quantized, `bmm` of two qint8 activations
+and `_softmax` run on the library's kernels, every other op dequantizes.  `F.linear` never reaches the table because the
+weight's `__torch_function__` intercepts first.
 """
 import ast
 
@@ -66,16 +66,9 @@ class ActivationQBytesTensor(QBytesTensor):
     def __torch_dispatch__(cls, op, types, args, kwargs=None):
         kwargs = dict(kwargs or {})
         packet = op.overloadpacket
-        if packet is torch.ops.aten.detach:
-            t = args[0]
-            return ActivationQBytesTensor(t.qtype, t.size(), t.stride(), packet(t._data), packet(t._scale))
-        if packet in (torch.ops.aten._to_copy, torch.ops.aten.to):
-            t = args[0]
-            dtype = kwargs.pop("dtype", t.dtype)
-            if dtype is not None and dtype != t.dtype:
-                raise ValueError("The dtype of an activations Tensor cannot be changed")
-            return ActivationQBytesTensor(t.qtype, t.size(), t.stride(), packet(t._data, **kwargs),
-                                          packet(t._scale, **kwargs))
+        qdispatch = activation_ops.get_qbytestensor_op_dispatch(packet)
+        if qdispatch is not None:
+            return qdispatch(*args, **kwargs)
         return qfallback(packet, *args, **kwargs)
 
 
@@ -83,3 +76,6 @@ def quantize_activation(t: torch.Tensor, qtype: qtype, scale: torch.Tensor):
     if scale.numel() != 1:
         raise ValueError("Parameter scale must be a scalar because activations can only be quantized per-tensor")
     return ActivationQBytesTensor.quantize(t, qtype, scale)
+
+
+from . import activation_ops  # noqa: E402  (the op table refers to the class above)
