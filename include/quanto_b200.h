@@ -184,6 +184,32 @@ QB200_API int64_t qb200_qbytes_bmm_workspace_bytes(int64_t batch, int64_t n, int
 QB200_API int qb200_qbytes_softmax(const void* x, const void* scale, const void* out_scale, void* out, int64_t rows,
                                    int64_t cols, int q_dtype, int scale_dtype, void* stream);
 
+/* ---- quantized 2-D convolution (the reference's QConv2d, optimum/quanto/nn/qconv2d.py) -------------------------- */
+
+/* out = F.conv2d(x, dequantize(W), bias, stride, padding, dilation) with groups == 1, as an implicit GEMM on the tensor
+ * cores (family 5): M = batch * Ho * Wo output pixels, N = cout, K = cin * kh * kw with k = c * kh * kw + r * kw + s.
+ * The weight [cout, cin, kh, kw] quantized along axis 0 is the linear weight [N, K] of qb200_qbits_mm (canonical packing,
+ * scale / shift [N * K / group]) and is dequantised in-kernel with the same arithmetic.  x: [batch, cin, h, w] and
+ * out: [batch, cout, Ho, Wo], both NCHW-contiguous in `dtype` (BF16 / F16), Ho = (h + 2 pad_h - dil_h (kh - 1) - 1) /
+ * stride_h + 1 (likewise Wo); zero padding.  bias: [cout] in `dtype` or NULL; out = rnd(conv + bias) with the bias
+ * added to the fp32 sum, the one rounding of the reference's QConv2d on the CPU (ATen's cuDNN path rounds the conv,
+ * then the bias add).  Nothing is allocated.
+ * QB200_ERR_ARG: bad shape or geometry, group not dividing K.  QB200_ERR_UNSUPPORTED: dtype F32, bits != 4, odd cout,
+ * K % 16 != 0, group neither a multiple of 32 nor K, M / N / K over int32, packed not 16-byte aligned, x / out / bias not
+ * aligned to their elements. */
+QB200_API int qb200_qbits_conv2d(const void* x, const uint8_t* packed, const void* scale, const void* shift,
+                                 const void* bias, void* out, int64_t batch, int64_t cin, int64_t h, int64_t w,
+                                 int64_t cout, int64_t kh, int64_t kw, int stride_h, int stride_w, int pad_h, int pad_w,
+                                 int dil_h, int dil_w, int group, int bits, int dtype, int shift_is_int, void* stream);
+
+/* The same for a weight-only 8-bit weight: W [cout, cin * kh * kw] of w_dtype in {I8, E4M3, E5M2, E4M3FNUZ} and
+ * scales [cout] in `dtype`; the weight operand is rnd(scale * W), as for qb200_qbytes_mm.  Same errors, with W
+ * (instead of packed) required 16-byte aligned. */
+QB200_API int qb200_qbytes_conv2d(const void* x, const void* w, const void* scales, const void* bias, void* out,
+                                  int64_t batch, int64_t cin, int64_t h, int64_t w_, int64_t cout, int64_t kh, int64_t kw,
+                                  int stride_h, int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int w_dtype,
+                                  int dtype, void* stream);
+
 /* ---- input gradient of the quantized linear (the backward's dX = gO @ W) ---------------------------------------- */
 
 /* grad_in[M, K] = grad_out[M, N] @ dequant(packed, scale, shift)[N, K] in one launch, reading the packed weights.
@@ -274,7 +300,8 @@ QB200_API int qb200_hqq_shrink(const void* x, void* out, int64_t numel, double b
 
 /* Which kernel family the last qb200_qbytes_mm / qb200_qbytes_bmm / qb200_qbits_mm / *_grad_input call on this thread dispatched to:
  * 0 none, 1 wgmma (TMA + warpgroup MMA), 2 CUDA-core (shape-agnostic), 3 warp-MMA gemv (int4, M <= 32: TMA ring or register streaming),
- * 4 byte-transpose pass + wgmma (qb200_qbytes_bmm with a B that is not K-contiguous).
+ * 4 byte-transpose pass + wgmma (qb200_qbytes_bmm with a B that is not K-contiguous), 5 implicit-GEMM convolution
+ * (qb200_qbits_conv2d / qb200_qbytes_conv2d).
  * For tests and bench accounting. */
 QB200_API int qb200_last_kernel_family(void);
 
@@ -291,7 +318,8 @@ QB200_API int qb200_last_kernel_family(void);
  *   key 7  int4 wgmma epilogue             : 1 ordinary stores (default: TMA stores from a shared-memory tile when the
  *                                            output is one dense [M, N] buffer with N % 16 == 0)
  *   key 8  qbytes_bmm route                : 2 CUDA-core kernel, 3 byte-transpose pass + wgmma for either B layout
- *                                            (default: wgmma reading a K-contiguous B in place) */
+ *                                            (default: wgmma reading a K-contiguous B in place)
+ *   key 9  conv2d tile rows                : 64 | 128 output pixels per tile */
 QB200_API int qb200_test_override(int key, int value);
 
 /* Developer aids.  They act only in a library built with `make KNOCKOUTS=1` (qb200_developer_build() == 1); in the

@@ -512,106 +512,14 @@ __device__ __forceinline__ void int4_epilogue(const GemmParams& p, const CUtenso
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// The kernel
-// ------------------------------------------------------------------------------------------------
+// The weight-staging warps of gemm_tc_kernel and conv_tc_kernel (conv_tc.cuh): int4 or 8-bit weights -> the stage's
+// 16-bit B tile, one staging group per stage slot (wgmma_pipe.cuh: StagingThread).
 template <class Cfg>
-__global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
-    gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                   const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
+__device__ __forceinline__ void stage_weights(const WgmmaPipe<typename Cfg::Pipe>& pipe, const GemmParams& p,
+                                              int num_tiles, int kblocks) {
   using L = typename Cfg::Pipe;
   constexpr int BN = Cfg::BN;
-
-  const auto pipe = WgmmaPipe<L>::init([&] {
-    tma_prefetch_desc(&tmap_a);
-    if constexpr (Cfg::BSRC == BSrc::TMA) tma_prefetch_desc(&tmap_b);
-    if constexpr (Cfg::BSRC == BSrc::INT4)
-      if (p.epi_tma) tma_prefetch_desc(&tmap_out);
-  });
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
-  constexpr int A_ELEM = (Cfg::KIND == MmaKind::F16 || Cfg::KIND == MmaKind::BF16) ? 2 : 1;
-  constexpr int KELEMS = Cfg::KBYTES / A_ELEM;  // K elements per stage
-  const int kblocks = (p.K + KELEMS - 1) / KELEMS;
-
-  if (warp < L::PRODUCER_WARP) {
-    // ------------------------------------------------------------------ consumers: wgmma + epilogue
-    const int wg = warp >> 2;
-    using AccT = typename std::conditional<Cfg::IS_INT, uint32_t, float>::type;
-    AccT acc[Cfg::NACC];
-    RingPos<L::NSTAGES> pos;
-    float s_ab = 0.f;
-    if constexpr (Cfg::BATCH) s_ab = scalar_scale_product(p.scales, p.scale_b, p.out_dt);
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m_blk = tile % p.num_m_blocks;
-      int n_blk = tile / p.num_m_blocks;
-      size_t out_base = 0;  // first element of the tile's batch in the output
-      if constexpr (Cfg::BATCH) {
-        const int b = n_blk / p.n_blocks_per_batch;
-        n_blk -= b * p.n_blocks_per_batch;
-        out_base = static_cast<size_t>(b) * p.M * p.ld;
-      }
-      pipe.consume_tile(pos, kblocks, acc, [&](uint32_t aa, uint32_t bb, bool accumulate) {
-        wgmma_slab<Cfg::KIND, BN>(acc, aa, bb, accumulate);
-      });
-      if constexpr (Cfg::BSRC == BSrc::INT4) {
-        int4_epilogue<typename Cfg::WT>(p, &tmap_out, acc, pipe.epi + wg * Cfg::EPI_TILE, m_blk * Cfg::BM + wg * 64,
-                                        n_blk, wg);
-      } else {
-        // epilogue straight from the fragment: thread holds rows r0 and r0 + 8, column pairs 8 j + 2 (lane % 4)
-        const int r0 = m_blk * Cfg::BM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = r0 + 8 * h;
-          if (row >= p.M) continue;
-          const size_t row_off = out_base + static_cast<size_t>(row) * p.ld + p.col0;
-#pragma unroll
-          for (int j = 0; j < BN / 8; ++j) {
-            const int n = n_blk * BN + 8 * j + 2 * (lane & 3);
-            if (n >= p.N) continue;
-            float f0, f1;
-            if constexpr (Cfg::IS_INT) {
-              f0 = __int2float_rn(static_cast<int>(acc[4 * j + 2 * h]));
-              f1 = __int2float_rn(static_cast<int>(acc[4 * j + 2 * h + 1]));
-            } else {
-              f0 = acc[4 * j + 2 * h];
-              f1 = acc[4 * j + 2 * h + 1];
-            }
-            if constexpr (Cfg::BATCH) {
-              f0 = __fmul_rn(f0, s_ab);
-              f1 = __fmul_rn(f1, s_ab);
-              epilogue_pair<false, false>(p, row_off, n, n + 1 < p.N, f0, f1);
-            } else {
-              epilogue_pair<Cfg::BSRC == BSrc::TMA || Cfg::BSRC == BSrc::F8>(p, row_off, n, n + 1 < p.N, f0, f1);
-            }
-          }
-        }
-      }
-    }
-    if constexpr (Cfg::BSRC == BSrc::INT4)
-      if ((threadIdx.x & 127) == 0) bulk_wait_group_all();  // the last tile's TMA store has completed
-    if (p.g.n_out > 1) __threadfence_system();  // this thread's peer stores are performed before the rank signals
-  } else if (warp == L::PRODUCER_WARP) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0 && Cfg::BSRC != BSrc::F8) {
-      constexpr uint32_t tx_bytes = Cfg::A_TILE + (Cfg::BSRC == BSrc::TMA ? Cfg::B_TILE : 0);
-      gather_wait_start(p.g);  // the activation may be the gathered output of the previous linear
-      pipe.produce(num_tiles, p.num_m_blocks, kblocks, tx_bytes, [&](uint8_t* dst, uint64_t* bar, int m_blk, int n_blk, int kb) {
-        if constexpr (Cfg::BATCH) {
-          const int b = n_blk / p.n_blocks_per_batch;
-          tma_load_3d(dst, &tmap_a, bar, kb * KELEMS, m_blk * Cfg::BM, b * p.a_batch_mul);
-          tma_load_3d(dst + Cfg::A_TILE, &tmap_b, bar, kb * KELEMS, (n_blk - b * p.n_blocks_per_batch) * BN,
-                      b * p.b_batch_mul);
-        } else {
-          tma_load_2d(dst, &tmap_a, bar, kb * KELEMS, m_blk * Cfg::BM);
-          if constexpr (Cfg::BSRC == BSrc::TMA) tma_load_2d(dst + Cfg::A_TILE, &tmap_b, bar, kb * KELEMS, n_blk * BN);
-        }
-      });
-    }
-  } else if constexpr (Cfg::BSRC == BSrc::INT4) {
+  if constexpr (Cfg::BSRC == BSrc::INT4) {
     // ------------------------------------------------------------------ weight staging: int4 -> WT tile
     StagingThread<L> sg(pipe, num_tiles, kblocks);
     const int r = sg.r;
@@ -623,7 +531,9 @@ __global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
     static_assert(ROWP == StagingThread<L>::GT, "one staging thread per packed row");
     const int half_n = p.N / 2;
     const int groups_per_row = p.K / p.group;
-    const bool two_sets = p.group < 64;  // group size 32: two (scale, shift) pairs per 64-k stage
+    // A group that is not a multiple of 64 (32, 96, 160, ...) can change at the middle of a 64-k stage: two (scale,
+    // shift) pairs per stage, one per 32-k half (a half lies inside one group: the group is a multiple of 32)
+    const bool two_sets = p.group % 64 != 0;
 
     struct Pre {
       uint4 raw[4];
@@ -640,7 +550,6 @@ __global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
 #pragma unroll
         for (int v = 0; v < 4; ++v)
           pr.raw[v] = (kbase + v * 16 < p.K) ? __ldg(reinterpret_cast<const uint4*>(src + v * 16)) : make_uint4(0, 0, 0, 0);
-        const int g0 = (p.group_log2 >= 0) ? (kbase >> p.group_log2) : (kbase / p.group);
 #pragma unroll
         for (int s = 0; s < 2; ++s) {
           if (s == 1 && !two_sets) break;
@@ -651,7 +560,9 @@ __global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
             pr.s_lo[1] = pr.s_lo[0]; pr.s_hi[1] = pr.s_hi[0]; pr.z_lo[1] = pr.z_lo[0]; pr.z_hi[1] = pr.z_hi[0];
             break;
           }
-          const size_t ilo = static_cast<size_t>(rp) * groups_per_row + g0 + s;
+          const int ks = kbase + 32 * s;  // first k of the half
+          const int gs = (p.group_log2 >= 0) ? (ks >> p.group_log2) : (ks / p.group);
+          const size_t ilo = static_cast<size_t>(rp) * groups_per_row + gs;
           const size_t ihi = ilo + static_cast<size_t>(half_n) * groups_per_row;
           const CoefPair c = load_coef_pair<ZP>(p.wscale, p.wshift, ilo, ihi);
           pr.s_lo[s] = bits_as<WT>(c.s_lo);
@@ -754,6 +665,110 @@ __global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
     // F8: one stage in registers at a time, the activation rows of the stage need the registers of a second buffer
     if constexpr (Cfg::BSRC == BSrc::F8) sg.template run_single<PreB>(load_pre, process);
     else sg.template run_ping_pong<PreB>(load_pre, process);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// The kernel
+// ------------------------------------------------------------------------------------------------
+template <class Cfg>
+__global__ void __launch_bounds__(Cfg::Pipe::NTHREADS, 1)
+    gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                   const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
+  using L = typename Cfg::Pipe;
+  constexpr int BN = Cfg::BN;
+
+  const auto pipe = WgmmaPipe<L>::init([&] {
+    tma_prefetch_desc(&tmap_a);
+    if constexpr (Cfg::BSRC == BSrc::TMA) tma_prefetch_desc(&tmap_b);
+    if constexpr (Cfg::BSRC == BSrc::INT4)
+      if (p.epi_tma) tma_prefetch_desc(&tmap_out);
+  });
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
+  constexpr int A_ELEM = (Cfg::KIND == MmaKind::F16 || Cfg::KIND == MmaKind::BF16) ? 2 : 1;
+  constexpr int KELEMS = Cfg::KBYTES / A_ELEM;  // K elements per stage
+  const int kblocks = (p.K + KELEMS - 1) / KELEMS;
+
+  if (warp < L::PRODUCER_WARP) {
+    // ------------------------------------------------------------------ consumers: wgmma + epilogue
+    const int wg = warp >> 2;
+    using AccT = typename std::conditional<Cfg::IS_INT, uint32_t, float>::type;
+    AccT acc[Cfg::NACC];
+    RingPos<L::NSTAGES> pos;
+    float s_ab = 0.f;
+    if constexpr (Cfg::BATCH) s_ab = scalar_scale_product(p.scales, p.scale_b, p.out_dt);
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int m_blk = tile % p.num_m_blocks;
+      int n_blk = tile / p.num_m_blocks;
+      size_t out_base = 0;  // first element of the tile's batch in the output
+      if constexpr (Cfg::BATCH) {
+        const int b = n_blk / p.n_blocks_per_batch;
+        n_blk -= b * p.n_blocks_per_batch;
+        out_base = static_cast<size_t>(b) * p.M * p.ld;
+      }
+      pipe.consume_tile(pos, kblocks, acc, [&](uint32_t aa, uint32_t bb, bool accumulate) {
+        wgmma_slab<Cfg::KIND, BN>(acc, aa, bb, accumulate);
+      });
+      if constexpr (Cfg::BSRC == BSrc::INT4) {
+        int4_epilogue<typename Cfg::WT>(p, &tmap_out, acc, pipe.epi + wg * Cfg::EPI_TILE, m_blk * Cfg::BM + wg * 64,
+                                        n_blk, wg);
+      } else {
+        // epilogue straight from the fragment: thread holds rows r0 and r0 + 8, column pairs 8 j + 2 (lane % 4)
+        const int r0 = m_blk * Cfg::BM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = r0 + 8 * h;
+          if (row >= p.M) continue;
+          const size_t row_off = out_base + static_cast<size_t>(row) * p.ld + p.col0;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int n = n_blk * BN + 8 * j + 2 * (lane & 3);
+            if (n >= p.N) continue;
+            float f0, f1;
+            if constexpr (Cfg::IS_INT) {
+              f0 = __int2float_rn(static_cast<int>(acc[4 * j + 2 * h]));
+              f1 = __int2float_rn(static_cast<int>(acc[4 * j + 2 * h + 1]));
+            } else {
+              f0 = acc[4 * j + 2 * h];
+              f1 = acc[4 * j + 2 * h + 1];
+            }
+            if constexpr (Cfg::BATCH) {
+              f0 = __fmul_rn(f0, s_ab);
+              f1 = __fmul_rn(f1, s_ab);
+              epilogue_pair<false, false>(p, row_off, n, n + 1 < p.N, f0, f1);
+            } else {
+              epilogue_pair<Cfg::BSRC == BSrc::TMA || Cfg::BSRC == BSrc::F8>(p, row_off, n, n + 1 < p.N, f0, f1);
+            }
+          }
+        }
+      }
+    }
+    if constexpr (Cfg::BSRC == BSrc::INT4)
+      if ((threadIdx.x & 127) == 0) bulk_wait_group_all();  // the last tile's TMA store has completed
+    if (p.g.n_out > 1) __threadfence_system();  // this thread's peer stores are performed before the rank signals
+  } else if (warp == L::PRODUCER_WARP) {
+    // ------------------------------------------------------------------ TMA producer
+    if (lane == 0 && Cfg::BSRC != BSrc::F8) {
+      constexpr uint32_t tx_bytes = Cfg::A_TILE + (Cfg::BSRC == BSrc::TMA ? Cfg::B_TILE : 0);
+      gather_wait_start(p.g);  // the activation may be the gathered output of the previous linear
+      pipe.produce(num_tiles, p.num_m_blocks, kblocks, tx_bytes, [&](uint8_t* dst, uint64_t* bar, int m_blk, int n_blk, int kb) {
+        if constexpr (Cfg::BATCH) {
+          const int b = n_blk / p.n_blocks_per_batch;
+          tma_load_3d(dst, &tmap_a, bar, kb * KELEMS, m_blk * Cfg::BM, b * p.a_batch_mul);
+          tma_load_3d(dst + Cfg::A_TILE, &tmap_b, bar, kb * KELEMS, (n_blk - b * p.n_blocks_per_batch) * BN,
+                      b * p.b_batch_mul);
+        } else {
+          tma_load_2d(dst, &tmap_a, bar, kb * KELEMS, m_blk * Cfg::BM);
+          if constexpr (Cfg::BSRC == BSrc::TMA) tma_load_2d(dst + Cfg::A_TILE, &tmap_b, bar, kb * KELEMS, n_blk * BN);
+        }
+      });
+    }
+  } else if constexpr (Cfg::BSRC != BSrc::TMA) {
+    stage_weights<Cfg>(pipe, p, num_tiles, kblocks);
   }
 
   __syncthreads();

@@ -93,7 +93,8 @@ enum : int { OVR_TILE_M = 0 /* 64 | 128 rows per wgmma tile; 256: the int4 swap-
              OVR_GEMV_SHAPE = 6 /* 2 = the two-CTAs-per-SM shape of the ring gemv (M <= 2) */,
              OVR_INT4_EPILOGUE = 7 /* 1 = the int4 wgmma epilogue stores without TMA */,
              OVR_BMM_ROUTE = 8 /* qbytes_bmm: 2 = CUDA-core kernel, 3 = K-major copy of B + wgmma for any B layout */,
-             OVR_COUNT = 9 };
+             OVR_CONV_TILE_M = 9 /* conv2d: 64 | 128 rows (output pixels) per tile */,
+             OVR_COUNT = 10 };
 // OVR_INT4_ROUTE values
 enum : int { ROUTE_AUTO = 0, ROUTE_INT4_GENERAL = 1, ROUTE_INT4_GEMV = 3, ROUTE_INT4_RING = 4, ROUTE_INT4_RING2 = 8 };
 // OVR_QBYTES_ROUTE values

@@ -21,8 +21,11 @@ namespace qb {
 
 // Warp roles and shared-memory budget from the kernel's tile choices.  TMA_ARRIVALS: arrivals of the TMA producer on
 // `full` per stage (0 when the staging warps write every operand); GROUP_WARPS: staging warps per stage slot;
-// EPI_BYTES: the consumers' output staging tiles, after the stages (a multiple of 1024 bytes, 0 when there are none).
-template <int MWG_, int NSTAGES_, int A_TILE_, int B_TILE_, int GROUP_WARPS_, int TMA_ARRIVALS_, int EPI_BYTES_ = 0>
+// EPI_BYTES: the consumers' output staging tiles, after the stages (a multiple of 1024 bytes, 0 when there are none);
+// GATHER_WARPS: warps after the staging warps that write every stage's A tile from registers (conv_tc.cuh), one arrive
+// on `full` each per stage -- they take the place of the TMA producer's arrive.
+template <int MWG_, int NSTAGES_, int A_TILE_, int B_TILE_, int GROUP_WARPS_, int TMA_ARRIVALS_, int EPI_BYTES_ = 0,
+          int GATHER_WARPS_ = 0>
 struct PipeLayout {
   static constexpr int MWG = MWG_;
   static constexpr int NSTAGES = NSTAGES_;
@@ -32,8 +35,10 @@ struct PipeLayout {
   static constexpr int NCVT_WARPS = NSTAGES * CVT_GROUP_WARPS;
   static constexpr int PRODUCER_WARP = 4 * MWG;
   static constexpr int FIRST_CVT_WARP = PRODUCER_WARP + 1;
-  static constexpr int NTHREADS = (FIRST_CVT_WARP + NCVT_WARPS) * 32;
-  static constexpr int FULL_ARRIVALS = TMA_ARRIVALS_ + CVT_GROUP_WARPS;
+  static constexpr int GATHER_WARPS = GATHER_WARPS_;
+  static constexpr int FIRST_GATHER_WARP = FIRST_CVT_WARP + NCVT_WARPS;
+  static constexpr int NTHREADS = (FIRST_GATHER_WARP + GATHER_WARPS) * 32;
+  static constexpr int FULL_ARRIVALS = TMA_ARRIVALS_ + CVT_GROUP_WARPS + GATHER_WARPS;
   static constexpr int EPI_BYTES = EPI_BYTES_;
   static_assert(EPI_BYTES % 1024 == 0, "output staging tiles keep the 1024-byte alignment of the swizzle");
   // 1024 bytes of alignment slack (the swizzled tiles need 1024-byte aligned bases) + the output staging + the barriers

@@ -61,11 +61,13 @@ EXPORTS = (
     "qb200_qbytes_bmm",
     "qb200_qbytes_bmm_workspace_bytes",
     "qb200_qbytes_softmax",
+    "qb200_qbits_conv2d",
+    "qb200_qbytes_conv2d",
 )
 
 # qb200_test_override keys (include/quanto_b200.h)
 (OVR_TILE_M, OVR_QBYTES_TILE_N, OVR_INT4_ROUTE, OVR_QBYTES_ROUTE, OVR_GEMV_PRODUCER, OVR_PDL, OVR_GEMV_SHAPE,
- OVR_INT4_EPILOGUE, OVR_BMM_ROUTE) = range(9)
+ OVR_INT4_EPILOGUE, OVR_BMM_ROUTE, OVR_CONV_TILE_M) = range(10)
 ROUTE_INT4_GENERAL, ROUTE_INT4_GEMV, ROUTE_INT4_RING, ROUTE_INT4_RING2 = 1, 3, 4, 8
 ROUTE_QBYTES_SIMT = 2
 ROUTE_BMM_SIMT, ROUTE_BMM_TRANSPOSE = 2, 3
@@ -152,6 +154,8 @@ def load():
         lib.qb200_qbytes_bmm_workspace_bytes.argtypes = [i64, i64, i64, i64, i32]
         lib.qb200_qbytes_bmm_workspace_bytes.restype = i64
         lib.qb200_qbytes_softmax.argtypes = [vp, vp, vp, vp, i64, i64, i32, i32, vp]
+        lib.qb200_qbits_conv2d.argtypes = [vp, vp, vp, vp, vp, vp] + [i64] * 7 + [i32] * 10 + [vp]
+        lib.qb200_qbytes_conv2d.argtypes = [vp, vp, vp, vp, vp] + [i64] * 7 + [i32] * 8 + [vp]
         for name in EXPORTS:
             getattr(lib, name)  # AttributeError here == header and library out of sync
         # Developer knock-outs exist only in a `make KNOCKOUTS=1` build and are set explicitly through

@@ -22,17 +22,21 @@ After this, every `optimum.quanto` object keeps working as before -- `quantize()
 4. `WeightQBytesLinearFunction.forward` (tensor/weights/qbytes.py:68-82) keeps calling `quanto::qbytes_mm`, with the bias
    fused into the kernel epilogue when there is one; its backward takes the input gradient from
    `quanto::qbytes_grad_input` the same way;
+5. `HqqOptimizer.__call__` (tensor/optimizers/hqq_optimizer.py:60-87 after affine_optimizer.py:27-64) runs
+   `quanto::quantize_qbits_hqq` -- two launches, no host synchronisation -- for a CUDA bf16 / fp16 weight quantized along
+   axis 0 to qint4 / qint2, and the reference's own code for everything else and whatever the kernel declines;
 6. `aten.bmm` and `aten._softmax` of the reference's `ActivationQBytesTensor` table
    (tensor/activations/qbytes_ops.py:175-186, 208-215) run on `quanto::qbytes_bmm` (an exact int8 x int8 product on the
    tensor cores instead of an fp32 bmm of int8 values cast to fp32) and `quanto::qbytes_softmax` (codes in, codes out,
-   one launch) for CUDA tensors; every case those entries decline falls through to the reference's own entry.
-5. `HqqOptimizer.__call__` (tensor/optimizers/hqq_optimizer.py:60-87 after affine_optimizer.py:27-64) runs
-   `quanto::quantize_qbits_hqq` -- two launches, no host synchronisation -- for a CUDA bf16 / fp16 weight quantized along
-   axis 0 to qint4 / qint2, and the reference's own code for everything else and whatever the kernel declines.
+   one launch) for CUDA tensors; every case those entries decline falls through to the reference's own entry;
+7. `F.conv2d` on the reference's `WeightQBitsTensor` / `WeightQBytesTensor` (its QConv2d, optimum/quanto/nn/qconv2d.py)
+   runs `quanto::qbits_conv2d` / `quanto::qbytes_conv2d` -- one implicit-GEMM launch -- when no graph is needed and the
+   kernel takes the problem, instead of qfallback's dense dequantised copy + cuDNN; everything else keeps the
+   reference's route.
 
 Used by tools/run_reference_tests.py to run the reference's OWN hot-path tests (tests/library, tests/tensor/ops,
 tests/nn/test_qlinear.py, and for 6 tests/tensor/ops/test_mm_dispatch.py, tests/tensor/activations/test_activations_dispatch.py,
-tests/nn/test_qattention.py) against these kernels.  Nothing here is imported by the rest of the package.
+tests/nn/test_qattention.py, for 7 tests/nn/test_qconv2d.py) against these kernels.  Nothing here is imported by the rest of the package.
 """
 import torch
 
@@ -191,4 +195,19 @@ def bind_reference():
 
     table[aten.bmm] = bmm
     table[aten._softmax] = softmax
+
+    # ---- 7. quantized conv2d: the package's own routing (library_conv.native_conv2d), for the reference's classes
+    from . import library_conv
+
+    def conv_torch_function(orig):
+        def torch_function(cls, func, types, args=(), kwargs=None):
+            if func is torch.nn.functional.conv2d:
+                out = library_conv.native_conv2d(args, kwargs or {}, RefQBits, RefQBytesW)
+                if out is not None:
+                    return out
+            return orig(cls, func, types, args, kwargs)
+        return classmethod(torch_function)
+
+    RefQBits.__torch_function__ = conv_torch_function(RefQBits.__torch_function__.__func__)
+    RefQBytesW.__torch_function__ = conv_torch_function(RefQBytesW.__torch_function__.__func__)
     _bound = True

@@ -1,9 +1,11 @@
-"""Quantized `torch.nn.Linear` (the caller of the hot path).
+"""Quantized `torch.nn.Linear` and `torch.nn.Conv2d` (the callers of the hot path).
 
 `QLinear.forward` is `F.linear(input, self.qweight, bias)` exactly as optimum/quanto/nn/qlinear.py:49-50; the
-weight's `__torch_function__` turns that into one `quanto::qbytes_mm` or `quanto::qbits_mm` launch.  `QModuleMixin`
-keeps the reference's constructor arguments, hooks, state-dict keys and freeze semantics
-(optimum/quanto/nn/qmodule.py:94-312).  QConv2d / QLayerNorm are out of scope (not linear).
+weight's `__torch_function__` turns that into one `quanto::qbytes_mm` or `quanto::qbits_mm` launch.  `QConv2d.forward`
+is `self._conv_forward(input, self.qweight, self.bias)` as optimum/quanto/nn/qconv2d.py; F.conv2d on a frozen weight
+becomes one `quanto::qbits_conv2d` / `quanto::qbytes_conv2d` launch where the kernel takes the problem.
+`QModuleMixin` keeps the reference's constructor arguments, hooks, state-dict keys and freeze semantics
+(optimum/quanto/nn/qmodule.py:94-312).
 """
 from typing import Optional, Union
 
@@ -14,7 +16,7 @@ from .tensor import (AbsmaxOptimizer, ActivationQBytesTensor, HqqOptimizer, MaxO
                      SymmetricOptimizer, PackedTensor, WeightQBitsTensor, WeightQBytesTensor, qint2, qint4, qtype, qtypes,
                      quantize_activation, quantize_weight)
 
-__all__ = ["QModuleMixin", "QLinear", "freeze"]
+__all__ = ["QModuleMixin", "QLinear", "QConv2d", "freeze"]
 
 
 def _pick_group_size(in_features: int) -> Optional[int]:
@@ -145,34 +147,53 @@ class QModuleMixin:
         exactly the default one, so the result equals `optimizer(...)` + `quantize_weight(...)` of the reference's
         CPU path bit for bit (nn/qmodule.py:245-266 with max_optimizer.py:26-37 / absmax_optimizer.py:29-36).
         Returns None when the composition of separate ops has to run instead.
+
+        A conv weight [Cout, Cin, kh, kw] is quantized as the linear weight [Cout, Cin * kh * kw] it flattens to (the
+        reference groups the row-major flattening, tensor/grouped.py); only the per-axis tensors are then given back the
+        4-D shapes the composition produces (packed [ceil(Cout / 2), Cin, kh, kw], scale / shift [Cout, 1, 1, 1]).
         """
         w = self.weight
-        if (w is None or not w.is_cuda or w.ndim != 2 or w.dtype not in (torch.float32, torch.float16, torch.bfloat16)
+        if (w is None or not w.is_cuda or w.ndim not in (2, 4)
+                or w.dtype not in (torch.float32, torch.float16, torch.bfloat16)
                 or (torch.is_grad_enabled() and w.requires_grad)):
             return None
+        w2 = w.detach().reshape(w.shape[0], -1)
+        coef_shape = (w.shape[0],) + (1,) * (w.ndim - 1)  # per-axis scales / shifts, as the optimizers keep them
         qt = self.weight_qtype
+
+        def qbits(packed, scale, shift):
+            group = self.weight_group_size or w2.shape[1]
+            rows = w.numel() // group
+            if self.weight_group_size is None and w.ndim == 4:
+                data = PackedTensor(packed.reshape((packed.shape[0],) + tuple(w.shape[1:])), qt.bits, w.size(),
+                                    w.stride())
+                scale, shift = scale.reshape(coef_shape), shift.reshape(coef_shape)
+            else:
+                data = PackedTensor(packed, qt.bits, torch.Size([rows, group]), (group, 1))
+            return WeightQBitsTensor(qt, 0, self.weight_group_size, w.size(), w.stride(), data, scale, shift)
+
         if qt in (qint2, qint4) and type(self.optimizer) is MaxOptimizer:
-            group = self.weight_group_size or w.shape[1]
+            group = self.weight_group_size or w2.shape[1]
             try:
-                packed, scale, shift = torch.ops.quanto.quantize_qbits_max(w.detach(), qt.bits, group, False)
+                packed, scale, shift = torch.ops.quanto.quantize_qbits_max(w2, qt.bits, group, False)
             except _native.UnsupportedConfiguration:
                 return None
-            rows = w.numel() // group
-            data = PackedTensor(packed, qt.bits, torch.Size([rows, group]), (group, 1))
-            return WeightQBitsTensor(qt, 0, self.weight_group_size, w.size(), w.stride(), data, scale, shift)
+            return qbits(packed, scale, shift)
         if qt in (qint2, qint4) and type(self.optimizer) is HqqOptimizer:
-            group = self.weight_group_size or w.shape[1]
-            fused = self.optimizer.fused(w.detach(), qt, 0, group)
+            if w.ndim == 4 and self.weight_group_size is None:
+                # per-axis HQQ reduces a whole [Cin, kh, kw] slice: the reference's float sums over the 4-D tensor run
+                # in another order than over the [Cout, K] rows the kernel reproduces, so its shifts may differ
+                return None
+            group = self.weight_group_size or w2.shape[1]
+            fused = self.optimizer.fused(w2, qt, 0, group)
             if fused is None:
                 return None
-            packed, scale, shift = fused
-            rows = w.numel() // group
-            data = PackedTensor(packed, qt.bits, torch.Size([rows, group]), (group, 1))
-            return WeightQBitsTensor(qt, 0, self.weight_group_size, w.size(), w.stride(), data, scale, shift)
+            return qbits(*fused)
         if (qt is not None and qt.bits == 8 and type(self.optimizer) is AbsmaxOptimizer and w.shape[0] > 1
                 and qt.dtype in (torch.int8, torch.float8_e4m3fn, torch.float8_e5m2)):
-            data, scale = torch.ops.quanto.quantize_qbytes_absmax(w.detach(), qt.dtype)
-            return WeightQBytesTensor(qt, 0, w.size(), w.stride(), data, scale, self.activation_qtype)
+            data, scale = torch.ops.quanto.quantize_qbytes_absmax(w2, qt.dtype)
+            return WeightQBytesTensor(qt, 0, w.size(), w.stride(), data.reshape(w.shape), scale.reshape(coef_shape),
+                                      self.activation_qtype)
         return None
 
     def quantize_input(self, module, input):
@@ -232,6 +253,23 @@ class QLinear(QModuleMixin, torch.nn.Linear):
         data = torch.ops.quanto.qbytes_linear_quantized(input._data, w._data, scales, self.bias, self.output_scale,
                                                         self.activation_qtype.dtype)
         return ActivationQBytesTensor(self.activation_qtype, data.size(), data.stride(), data, self.output_scale)
+
+
+class QConv2d(QModuleMixin, torch.nn.Conv2d):
+    """optimum/quanto/nn/qconv2d.py: the weight is quantized along axis 0 with the group size of its flattening
+    Cin * kh * kw; the input is not quantized (quantize_input stays False), the output is when `activations` is set."""
+
+    @classmethod
+    def qcreate(cls, module, weights: qtype, activations: Optional[qtype] = None,
+                optimizer: Optional[Optimizer] = None, device: Optional[torch.device] = None):
+        return cls(in_channels=module.in_channels, out_channels=module.out_channels, kernel_size=module.kernel_size,
+                   stride=module.stride, padding=module.padding, dilation=module.dilation, groups=module.groups,
+                   bias=module.bias is not None, padding_mode=module.padding_mode, dtype=module.weight.dtype,
+                   device=device, weights=weights, activations=activations, optimizer=optimizer)
+
+    def forward(self, input: torch.Tensor) -> torch.Tensor:
+        # a padding_mode other than 'zeros' pads with F.pad here, then the conv itself runs with padding 0
+        return self._conv_forward(input, self.qweight, self.bias)
 
 
 def freeze(model: torch.nn.Module):

@@ -112,6 +112,10 @@ class WeightQBytesTensor(QBytesTensor):
         kwargs = kwargs or {}
         if func is torch.nn.functional.linear:
             return WeightQBytesLinearFunction.apply(*_linear_args(*args, **kwargs))
+        if func is torch.nn.functional.conv2d:
+            out = _native_conv2d(args, kwargs)
+            if out is not None:
+                return out
         if func is torch.equal:
             return args[0].equal(args[1])
         with torch._C.DisableTorchFunctionSubclass():
@@ -277,6 +281,10 @@ class WeightQBitsTensor(QBitsTensor):
             if isinstance(other, WeightQBitsTensor) and other._fused_linear_ok(input):
                 return WeightQBitsLinearFunction.apply(input, other, bias)
             return QuantizedLinearFunction.apply(input, other, bias)
+        if func is torch.nn.functional.conv2d:
+            out = _native_conv2d(args, kwargs)
+            if out is not None:
+                return out
         if func is torch.equal:
             return args[0].equal(args[1])
         with torch._C.DisableTorchFunctionSubclass():
@@ -309,6 +317,14 @@ def _linear_args(input, weight=None, bias=None, **kw):
     if "bias" in kw:
         bias = kw["bias"]
     return input, weight, bias
+
+
+def _native_conv2d(args, kwargs):
+    """F.conv2d on a quantized weight as one quanto::qbits_conv2d / quanto::qbytes_conv2d launch, or None: the caller then
+    runs the reference's composition (library_conv.native_conv2d)."""
+    from .. import library_conv
+
+    return library_conv.native_conv2d(args, kwargs, WeightQBitsTensor, WeightQBytesTensor)
 
 
 def quantize_weight(t, qtype, axis, scale, shift=None, group_size=None, activation_qtype=None, optimized=True):
