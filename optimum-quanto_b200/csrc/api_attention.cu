@@ -10,8 +10,6 @@
 //                         (:208-215) in one launch: 8-bit codes in, 8-bit codes out.
 #include "../../include/quanto_b200.h"
 
-#include <cstring>
-
 #include "gemm_tc.cuh"
 #include "host_common.cuh"
 
@@ -114,17 +112,12 @@ __global__ void __launch_bounds__(256)
     }
 }
 
+// the batched configuration of the int8 x int8 wgmma GEMM (int8 only)
 template <int MWG, int BN>
-static int launch_bmm_tc(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t st) {
-  using Cfg = GemmCfg<MmaKind::I8, BSrc::TMA, MWG, BN, __nv_bfloat16, false, 0, 0, true>;
-  CUtensorMap tout;
-  std::memset(&tout, 0, sizeof(tout));  // the epilogue stores straight from the accumulators
-  return launch_persistent<gemm_tc_kernel<Cfg>, typename Cfg::Pipe>(p.num_m_blocks * p.num_n_blocks, st,
-                                                                    "qbytes_bmm wgmma launch", ta, tb, tout, p);
-}
+using BmmCfg = GemmCfg<MmaKind::I8, BSrc::TMA, MWG, BN, __nv_bfloat16, false, 0, 0, true>;
 
 static bool bmm_tc_shape_ok(const void* a, int64_t m, int64_t n, int64_t k, int64_t a_bs) {
-  return k % 16 == 0 && reinterpret_cast<uintptr_t>(a) % 16 == 0 && a_bs % 16 == 0 && m <= INT32_MAX &&
+  return k % 16 == 0 && aligned16(a) && a_bs % 16 == 0 && m <= INT32_MAX &&
          n <= INT32_MAX && k <= INT32_MAX;
 }
 
@@ -164,7 +157,7 @@ static int qbytes_bmm_impl(const void* a, const void* b, const void* sa, const v
   if (rc != OK) return rc;
   const int route = test_override(OVR_BMM_ROUTE);
   const bool copy = bmm_needs_copy(b_layout);
-  const bool b_in_place_ok = reinterpret_cast<uintptr_t>(b) % 16 == 0 && b_bs % 16 == 0;
+  const bool b_in_place_ok = aligned16(b) && b_bs % 16 == 0;
   const int tile_m = wgmma_tile_m(m);
   const int64_t mb = (m + tile_m - 1) / tile_m;
   if (route != ROUTE_BMM_SIMT && bmm_tc_shape_ok(a, m, n, k, a_bs) && (copy || b_in_place_ok) &&
@@ -172,7 +165,7 @@ static int qbytes_bmm_impl(const void* a, const void* b, const void* sa, const v
     const void* bk = b;
     int64_t bk_bs = b_bs;
     if (copy) {
-      if (ws == nullptr || ws_bytes < bmm_copy_bytes(batch, n, k, b_bs) || reinterpret_cast<uintptr_t>(ws) % 16 != 0)
+      if (ws == nullptr || ws_bytes < bmm_copy_bytes(batch, n, k, b_bs) || !aligned16(ws))
         return fail(ERR_ARG, "qbytes_bmm: the K-major copy of B needs qb200_qbytes_bmm_workspace_bytes() bytes of "
                              "16-byte aligned workspace");
       const int copies = b_bs == 0 ? 1 : static_cast<int>(batch);
@@ -193,18 +186,9 @@ static int qbytes_bmm_impl(const void* a, const void* b, const void* sa, const v
     int bn = (tile_m == 128 && waves(256) <= waves(128)) ? 256 : 128;
     const int force_bn = test_override(OVR_QBYTES_TILE_N);
     if (force_bn == 128 || force_bn == 256) bn = force_bn;
-    GemmParams p{};
+    GemmParams p = dense_gemm_params(out, nullptr, dt, m, n, k);
     p.scales = sa;
     p.scale_b = sb;
-    p.out = out;
-    p.g.out_peer[0] = out;
-    p.g.n_out = 1;
-    p.g.world = 1;
-    p.ld = static_cast<int>(n);
-    p.out_dt = dt;
-    p.M = static_cast<int>(m);
-    p.N = static_cast<int>(n);
-    p.K = static_cast<int>(k);
     p.num_m_blocks = static_cast<int>(mb);
     p.n_blocks_per_batch = static_cast<int>((n + bn - 1) / bn);
     p.num_n_blocks = static_cast<int>(batch) * p.n_blocks_per_batch;
@@ -216,8 +200,10 @@ static int qbytes_bmm_impl(const void* a, const void* b, const void* sa, const v
     rc = make_tmap_3d_bytes(&tb, bk, bk_bs == 0 ? 1 : batch, n, k, bk_bs == 0 ? n * k : bk_bs, bn);
     if (rc != OK) return rc;
     set_kernel_family(copy ? 4 : 1);
-    if (tile_m == 64) return bn == 256 ? launch_bmm_tc<1, 256>(ta, tb, p, st) : launch_bmm_tc<1, 128>(ta, tb, p, st);
-    return bn == 256 ? launch_bmm_tc<2, 256>(ta, tb, p, st) : launch_bmm_tc<2, 128>(ta, tb, p, st);
+    return dispatch_mwg(tile_m, [&](auto MWG) {
+      if (bn == 256) return launch_gemm_tc<BmmCfg<MWG, 256>>(&ta, &tb, nullptr, p, st, "qbytes_bmm wgmma launch");
+      return launch_gemm_tc<BmmCfg<MWG, 128>>(&ta, &tb, nullptr, p, st, "qbytes_bmm wgmma launch");
+    });
   }
   if (batch > 65535 || (m + kST - 1) / kST > 65535)
     return fail(ERR_UNSUPPORTED, "qbytes_bmm: the CUDA-core kernel takes at most 65535 batches of 65535 x 64 rows");

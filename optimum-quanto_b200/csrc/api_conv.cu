@@ -43,16 +43,7 @@ static int conv_setup(const char* what, const ConvArgs& a, GemmParams* p, ConvGe
   if (reinterpret_cast<uintptr_t>(a.x) % 2 != 0 || reinterpret_cast<uintptr_t>(a.out) % 2 != 0 ||
       reinterpret_cast<uintptr_t>(a.bias) % 2 != 0)
     return fail(ERR_UNSUPPORTED, "%s: input, bias and output must be aligned to their elements", what);
-  *p = GemmParams{};
-  p->bias = a.bias;
-  p->out = a.out;
-  p->g.out_peer[0] = a.out;
-  p->g.n_out = 1;
-  p->g.world = 1;
-  p->out_dt = a.dtype;
-  p->M = static_cast<int>(m);
-  p->N = static_cast<int>(a.cout);
-  p->K = static_cast<int>(k);
+  *p = dense_gemm_params(a.out, a.bias, a.dtype, m, a.cout, k);
   p->dbg = debug_flags();
   *g = ConvGeom{a.x, static_cast<int>(a.cin), static_cast<int>(a.h), static_cast<int>(a.w), static_cast<int>(ho),
                 static_cast<int>(wo), static_cast<int>(a.kh), static_cast<int>(a.kw), a.sh, a.sw, a.ph, a.pw, a.dh, a.dw};
@@ -68,33 +59,6 @@ static int conv_tile_m(GemmParams* p, int64_t n_tiles) {
   p->num_m_blocks = (p->M + t - 1) / t;
   p->num_n_blocks = static_cast<int>(n_tiles);
   return t;
-}
-
-template <int MWG>
-static int launch_conv_int4(const GemmParams& p, const ConvGeom& g, int dtype, bool zp, cudaStream_t st) {
-  constexpr int BN = 128;
-  if (dtype == DT_BF16) {
-    if (zp) return launch_conv<GemmCfg<MmaKind::BF16, BSrc::INT4, MWG, BN, __nv_bfloat16, true>>(p, g, st);
-    return launch_conv<GemmCfg<MmaKind::BF16, BSrc::INT4, MWG, BN, __nv_bfloat16, false>>(p, g, st);
-  }
-  if (zp) return launch_conv<GemmCfg<MmaKind::F16, BSrc::INT4, MWG, BN, __half, true>>(p, g, st);
-  return launch_conv<GemmCfg<MmaKind::F16, BSrc::INT4, MWG, BN, __half, false>>(p, g, st);
-}
-
-template <int MWG>
-static int launch_conv_bytes(const GemmParams& p, const ConvGeom& g, int dtype, int wk, cudaStream_t st) {
-  constexpr int BN = 128;
-  using BF = __nv_bfloat16;
-  if (dtype == DT_BF16) {
-    if (wk == 0) return launch_conv<GemmCfg<MmaKind::BF16, BSrc::BYTES, MWG, BN, BF, false, 0>>(p, g, st);
-    if (wk == 1) return launch_conv<GemmCfg<MmaKind::BF16, BSrc::BYTES, MWG, BN, BF, false, 1>>(p, g, st);
-    if (wk == 2) return launch_conv<GemmCfg<MmaKind::BF16, BSrc::BYTES, MWG, BN, BF, false, 2>>(p, g, st);
-    return launch_conv<GemmCfg<MmaKind::BF16, BSrc::BYTES, MWG, BN, BF, false, 3>>(p, g, st);
-  }
-  if (wk == 0) return launch_conv<GemmCfg<MmaKind::F16, BSrc::BYTES, MWG, BN, __half, false, 0>>(p, g, st);
-  if (wk == 1) return launch_conv<GemmCfg<MmaKind::F16, BSrc::BYTES, MWG, BN, __half, false, 1>>(p, g, st);
-  if (wk == 2) return launch_conv<GemmCfg<MmaKind::F16, BSrc::BYTES, MWG, BN, __half, false, 2>>(p, g, st);
-  return launch_conv<GemmCfg<MmaKind::F16, BSrc::BYTES, MWG, BN, __half, false, 3>>(p, g, st);
 }
 
 }  // namespace qb
@@ -120,7 +84,7 @@ int qb200_qbits_conv2d(const void* x, const uint8_t* packed, const void* scale, 
   // a 32-k half of a stage must lie inside one group (conv_tc.cuh); one group per row (per-axis) always does
   if (group % 32 != 0 && group != p.K)
     return fail(ERR_UNSUPPORTED, "qbits_conv2d: group %d is neither a multiple of 32 nor K", group);
-  if (reinterpret_cast<uintptr_t>(packed) % 16 != 0) return fail(ERR_UNSUPPORTED, "qbits_conv2d: packed weights not 16-byte aligned");
+  if (!aligned16(packed)) return fail(ERR_UNSUPPORTED, "qbits_conv2d: packed weights not 16-byte aligned");
   if (p.M == 0) return OK;
   rc = check_arch();
   if (rc != OK) return rc;
@@ -132,8 +96,12 @@ int qb200_qbits_conv2d(const void* x, const uint8_t* packed, const void* scale, 
   p.shift_is_int = shift_is_int;
   const int t = conv_tile_m(&p, (cout / 2 + 63) / 64);
   set_kernel_family(5);
-  if (t == 64) return launch_conv_int4<1>(p, g, dtype, shift_is_int != 0, a.stream);
-  return launch_conv_int4<2>(p, g, dtype, shift_is_int != 0, a.stream);
+  return dispatch_act16_zp(dtype, shift_is_int, [&](auto act, auto ZP) {
+    return dispatch_mwg(t, [&](auto MWG) {
+      using A = decltype(act);
+      return launch_conv<GemmCfg<A::KIND, BSrc::INT4, MWG, 128, typename A::WT, ZP>>(p, g, a.stream);
+    });
+  });
 }
 
 int qb200_qbytes_conv2d(const void* x, const void* wq, const void* scales, const void* bias, void* out, int64_t batch,
@@ -148,7 +116,7 @@ int qb200_qbytes_conv2d(const void* x, const void* wq, const void* scales, const
   ConvGeom g;
   int rc = conv_setup("qbytes_conv2d", a, &p, &g);
   if (rc != OK) return rc;
-  if (reinterpret_cast<uintptr_t>(wq) % 16 != 0) return fail(ERR_UNSUPPORTED, "qbytes_conv2d: weights not 16-byte aligned");
+  if (!aligned16(wq)) return fail(ERR_UNSUPPORTED, "qbytes_conv2d: weights not 16-byte aligned");
   if (p.M == 0) return OK;
   rc = check_arch();
   if (rc != OK) return rc;
@@ -156,10 +124,15 @@ int qb200_qbytes_conv2d(const void* x, const void* wq, const void* scales, const
   p.wscale = scales;
   p.w_dt = w_dtype;
   const int t = conv_tile_m(&p, (cout + 127) / 128);
-  const int wk = (w_dtype == DT_I8) ? 0 : (w_dtype == DT_E4M3 ? 1 : (w_dtype == DT_E5M2 ? 2 : 3));
   set_kernel_family(5);
-  if (t == 64) return launch_conv_bytes<1>(p, g, dtype, wk, a.stream);
-  return launch_conv_bytes<2>(p, g, dtype, wk, a.stream);
+  return dispatch_act16(dtype, [&](auto act) {
+    return dispatch_wkind(w_dtype, [&](auto WK) {
+      return dispatch_mwg(t, [&](auto MWG) {
+        using A = decltype(act);
+        return launch_conv<GemmCfg<A::KIND, BSrc::BYTES, MWG, 128, typename A::WT, false, WK>>(p, g, a.stream);
+      });
+    });
+  });
 }
 
 }  // extern "C"

@@ -138,7 +138,7 @@ static int encode_2d(CUtensorMap* map, const void* base, int dt, int64_t rows, i
     case DT_F32: type = CU_TENSOR_MAP_DATA_TYPE_FLOAT32; esz = 4; break;
     default: type = CU_TENSOR_MAP_DATA_TYPE_UINT8; esz = 1; break;
   }
-  if (reinterpret_cast<uintptr_t>(base) % 16 != 0) return fail(ERR_ARG, "TMA operand not 16-byte aligned");
+  if (!aligned16(base)) return fail(ERR_ARG, "TMA operand not 16-byte aligned");
   if ((pitch_elems * esz) % 16 != 0)
     return fail(ERR_ARG, "TMA row pitch %lld not a multiple of 16 bytes", (long long)(pitch_elems * esz));
   const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
@@ -160,7 +160,7 @@ int make_tmap_planes(CUtensorMap* map, const void* base, int dt, int64_t rows, i
   EncodeTiledFn enc = get_encode_fn();
   if (enc == nullptr) return fail(ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
   if (dt != DT_BF16 && dt != DT_F16) return fail(ERR_ARG, "plane tensor map: 16-bit elements only");
-  if (reinterpret_cast<uintptr_t>(base) % 16 != 0) return fail(ERR_ARG, "TMA operand not 16-byte aligned");
+  if (!aligned16(base)) return fail(ERR_ARG, "TMA operand not 16-byte aligned");
   if (cols % 16 != 0) return fail(ERR_ARG, "plane tensor map: cols %lld not a multiple of 16", (long long)cols);
   const CUtensorMapDataType type = dt == DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const cuuint64_t half = static_cast<cuuint64_t>(cols / 2);
@@ -182,7 +182,7 @@ int make_tmap_3d_bytes(CUtensorMap* map, const void* base, int64_t batch, int64_
                        int64_t batch_stride, int box_rows) {
   EncodeTiledFn enc = get_encode_fn();
   if (enc == nullptr) return fail(ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  if (reinterpret_cast<uintptr_t>(base) % 16 != 0) return fail(ERR_ARG, "TMA operand not 16-byte aligned");
+  if (!aligned16(base)) return fail(ERR_ARG, "TMA operand not 16-byte aligned");
   if (cols % 16 != 0 || batch_stride % 16 != 0)
     return fail(ERR_ARG, "TMA row pitch %lld / batch stride %lld not a multiple of 16 bytes", (long long)cols,
                 (long long)batch_stride);
@@ -195,12 +195,6 @@ int make_tmap_3d_bytes(CUtensorMap* map, const void* base, int64_t batch, int64_
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(ERR_CUDA, "cuTensorMapEncodeTiled (3-d) failed with CUresult %d", static_cast<int>(r));
   return OK;
-}
-
-int make_tmap_2d_view(CUtensorMap* map, const void* base, int dt, int64_t rows, int64_t cols, int64_t pitch_elems,
-                      int box_cols, int box_rows, bool swizzle128) {
-  return encode_2d(map, base, dt, rows, cols, pitch_elems, box_cols, box_rows,
-                   swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE);
 }
 
 }  // namespace qb

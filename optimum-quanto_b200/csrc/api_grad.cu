@@ -13,30 +13,10 @@ static int launch_dgrad(const CUtensorMap& tg, const DgradParams& p, cudaStream_
                                                                        "gemm_dgrad_kernel launch", tg, p);
 }
 
-static bool aligned16(const void* ptr) { return reinterpret_cast<uintptr_t>(ptr) % 16 == 0; }
-
 // The autograd engine runs a CUDA backward on a thread of its own, where no context may be current yet: the driver's
 // tensor-map encoder (unlike the runtime calls) then fails with CUDA_ERROR_INVALID_CONTEXT.  cudaSetDevice makes the
 // device's primary context current on the calling thread.
 static int make_context_current() { return check_cuda(cudaSetDevice(current_device()), "cudaSetDevice"); }
-
-template <int MWG>
-static int launch_dgrad_int4(const CUtensorMap& tg, const DgradParams& p, int dtype, bool zp, cudaStream_t st) {
-  if (dtype == DT_BF16) {
-    if (zp) return launch_dgrad<DgradCfg<true, MWG, __nv_bfloat16, true>>(tg, p, st);
-    return launch_dgrad<DgradCfg<true, MWG, __nv_bfloat16, false>>(tg, p, st);
-  }
-  if (zp) return launch_dgrad<DgradCfg<true, MWG, __half, true>>(tg, p, st);
-  return launch_dgrad<DgradCfg<true, MWG, __half, false>>(tg, p, st);
-}
-
-template <int MWG, typename WT>
-static int launch_dgrad_bytes(const CUtensorMap& tg, const DgradParams& p, int w_dtype, cudaStream_t st) {
-  if (w_dtype == DT_I8) return launch_dgrad<DgradCfg<false, MWG, WT, false, 0>>(tg, p, st);
-  if (w_dtype == DT_E4M3) return launch_dgrad<DgradCfg<false, MWG, WT, false, 1>>(tg, p, st);
-  if (w_dtype == DT_E5M2) return launch_dgrad<DgradCfg<false, MWG, WT, false, 2>>(tg, p, st);
-  return launch_dgrad<DgradCfg<false, MWG, WT, false, 3>>(tg, p, st);
-}
 
 static int qbits_grad_input_impl(const void* grad_out, const uint8_t* packed, const void* scale, const void* shift,
                                  void* grad_in, int64_t m, int64_t n, int64_t k, int group, int dtype, int shift_is_int,
@@ -75,9 +55,11 @@ static int qbits_grad_input_impl(const void* grad_out, const uint8_t* packed, co
   rc = make_tmap_planes(&tg, grad_out, dtype, m, n, tile_m);
   if (rc != OK) return rc;
   set_kernel_family(1);
-  const bool zp = shift_is_int != 0;
-  if (tile_m == 64) return launch_dgrad_int4<1>(tg, p, dtype, zp, stream);
-  return launch_dgrad_int4<2>(tg, p, dtype, zp, stream);
+  return dispatch_act16_zp(dtype, shift_is_int, [&](auto act, auto ZP) {
+    return dispatch_mwg(tile_m, [&](auto MWG) {
+      return launch_dgrad<DgradCfg<true, MWG, typename decltype(act)::WT, ZP>>(tg, p, stream);
+    });
+  });
 }
 
 static int qbytes_grad_input_impl(const void* grad_out, const void* w, const void* scales, void* grad_in, int64_t m,
@@ -113,12 +95,13 @@ static int qbytes_grad_input_impl(const void* grad_out, const void* w, const voi
   rc = make_tmap_2d(&tg, grad_out, dtype, m, n, tile_m);
   if (rc != OK) return rc;
   set_kernel_family(1);
-  if (dtype == DT_BF16) {
-    if (tile_m == 64) return launch_dgrad_bytes<1, __nv_bfloat16>(tg, p, w_dtype, stream);
-    return launch_dgrad_bytes<2, __nv_bfloat16>(tg, p, w_dtype, stream);
-  }
-  if (tile_m == 64) return launch_dgrad_bytes<1, __half>(tg, p, w_dtype, stream);
-  return launch_dgrad_bytes<2, __half>(tg, p, w_dtype, stream);
+  return dispatch_act16(dtype, [&](auto act) {
+    return dispatch_wkind(w_dtype, [&](auto WK) {
+      return dispatch_mwg(tile_m, [&](auto MWG) {
+        return launch_dgrad<DgradCfg<false, MWG, typename decltype(act)::WT, false, WK>>(tg, p, stream);
+      });
+    });
+  });
 }
 
 }  // namespace qb

@@ -12,44 +12,11 @@ namespace qb {
 int launch_qbits_mm_simt(const void*, const uint8_t*, const void*, const void*, const void*, void*, int, int, int, int,
                          int, int, int, int64_t, int64_t, cudaStream_t);
 
-template <class Cfg>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tout, const GemmParams& p, cudaStream_t stream) {
-  CUtensorMap tb;
-  std::memset(&tb, 0, sizeof(tb));  // the weight tile is staged by the kernel's own warps
-  return launch_persistent<gemm_tc_kernel<Cfg>, typename Cfg::Pipe>(p.num_m_blocks * p.num_n_blocks, stream,
-                                                                    "gemm_tc_kernel launch", ta, tb, tout, p);
-}
-
-template <int MWG>
-static int launch_int4(const CUtensorMap& ta, const CUtensorMap& tout, const GemmParams& p, int dtype, bool zp,
-                       cudaStream_t st) {
-  constexpr int BN = 128;
-  if (dtype == DT_BF16) {
-    if (zp) return launch_gemm<GemmCfg<MmaKind::BF16, BSrc::INT4, MWG, BN, __nv_bfloat16, true>>(ta, tout, p, st);
-    return launch_gemm<GemmCfg<MmaKind::BF16, BSrc::INT4, MWG, BN, __nv_bfloat16, false>>(ta, tout, p, st);
-  }
-  if (zp) return launch_gemm<GemmCfg<MmaKind::F16, BSrc::INT4, MWG, BN, __half, true>>(ta, tout, p, st);
-  return launch_gemm<GemmCfg<MmaKind::F16, BSrc::INT4, MWG, BN, __half, false>>(ta, tout, p, st);
-}
-
-template <int T>
-static int launch_w4(const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tout, const GemmParams& p,
-                     int dtype, bool zp, cudaStream_t st) {
-  const int tiles = p.num_m_blocks * p.num_n_blocks;
-  if (dtype == DT_BF16) {
-    if (zp) {
-      using C = W4Cfg<MmaKind::BF16, T, __nv_bfloat16, true>;
-      return launch_persistent<gemm_w4_kernel<C>, C>(tiles, st, "gemm_w4_kernel launch", ta, tw, tout, p);
-    }
-    using C = W4Cfg<MmaKind::BF16, T, __nv_bfloat16, false>;
-    return launch_persistent<gemm_w4_kernel<C>, C>(tiles, st, "gemm_w4_kernel launch", ta, tw, tout, p);
-  }
-  if (zp) {
-    using C = W4Cfg<MmaKind::F16, T, __half, true>;
-    return launch_persistent<gemm_w4_kernel<C>, C>(tiles, st, "gemm_w4_kernel launch", ta, tw, tout, p);
-  }
-  using C = W4Cfg<MmaKind::F16, T, __half, false>;
-  return launch_persistent<gemm_w4_kernel<C>, C>(tiles, st, "gemm_w4_kernel launch", ta, tw, tout, p);
+template <class C>
+static int launch_gemm_w4(const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tout, const GemmParams& p,
+                          cudaStream_t st) {
+  return launch_persistent<gemm_w4_kernel<C>, C>(p.num_m_blocks * p.num_n_blocks, st, "gemm_w4_kernel launch", ta, tw,
+                                                 tout, p);
 }
 
 // Which int4 wgmma kernel runs a problem of m_blocks 128-token blocks and half_n packed rows.  The swap-AB kernel
@@ -97,8 +64,7 @@ static int qbits_mm_impl(QbitsArgs& q) {
   // tensor-core kernels: 4-bit, 16-bit activations, N even, K % 16 == 0, group 32 or a multiple of 64, aligned buffers.
   // Everything else runs on the shape-agnostic CUDA-core kernel (same operands, same rounding order).
   const bool tc_ok = q.bits == 4 && (dtype == DT_BF16 || dtype == DT_F16) && n % 2 == 0 && k % 16 == 0 &&
-                     (group == 32 || group % 64 == 0) && reinterpret_cast<uintptr_t>(q.packed) % 16 == 0 &&
-                     reinterpret_cast<uintptr_t>(q.out) % 16 == 0 && reinterpret_cast<uintptr_t>(q.a) % 16 == 0;
+                     (group == 32 || group % 64 == 0) && aligned16(q.packed) && aligned16(q.out) && aligned16(q.a);
   if (!tc_ok) {
     if (gathered) return fail(ERR_UNSUPPORTED, "qbits_mm_gather: the fused gather exists for the tensor-core kernels only");
     set_kernel_family(2);
@@ -112,17 +78,10 @@ static int qbits_mm_impl(QbitsArgs& q) {
   rc = qbits_small_dispatch(q, &handled);
   if (rc != OK || handled) return rc;
 
-  GemmParams p{};
-  p.scales = nullptr;
-  p.bias = q.bias;
-  p.out = q.out;
-  p.g = q.g;
+  GemmParams p = dense_gemm_params(q.out, q.bias, dtype, m, n, k);
+  p.g = q.g;  // the fused gather's peer buffers and column slab
   p.ld = static_cast<int>(q.ld);
   p.col0 = static_cast<int>(q.col0);
-  p.out_dt = dtype;
-  p.M = static_cast<int>(m);
-  p.N = static_cast<int>(n);
-  p.K = static_cast<int>(k);
   p.wq = q.packed;
   p.wscale = q.scale;
   p.wshift = q.shift;
@@ -155,19 +114,22 @@ static int qbits_mm_impl(QbitsArgs& q) {
   std::memset(&tout, 0, sizeof(tout));
   p.epi_tma = 0;
   if (test_override(OVR_INT4_EPILOGUE) != 1 && q.g.n_out == 1 && q.g.out_peer[0] == q.out && q.ld == n && q.col0 == 0 &&
-      n % 16 == 0 && reinterpret_cast<uintptr_t>(q.out) % 16 == 0) {
+      n % 16 == 0 && aligned16(q.out)) {
     if (make_tmap_planes(&tout, q.out, dtype, m, n, swap ? t : 64) == OK) p.epi_tma = 1;
     else std::memset(&tout, 0, sizeof(tout));
   }
   set_kernel_family(1);
-  const bool zp = q.shift_is_int != 0;
-  if (!swap) {
-    if (tile_m == 64) return launch_int4<1>(ta, tout, p, dtype, zp, q.stream);
-    return launch_int4<2>(ta, tout, p, dtype, zp, q.stream);
-  }
-  if (t == 64) return launch_w4<64>(ta, tw, tout, p, dtype, zp, q.stream);
-  if (t == 128) return launch_w4<128>(ta, tw, tout, p, dtype, zp, q.stream);
-  return launch_w4<256>(ta, tw, tout, p, dtype, zp, q.stream);
+  return dispatch_act16_zp(dtype, q.shift_is_int, [&](auto act, auto ZP) {
+    using A = decltype(act);
+    if (!swap)
+      return dispatch_mwg(tile_m, [&](auto MWG) {
+        return launch_gemm_tc<GemmCfg<A::KIND, BSrc::INT4, MWG, 128, typename A::WT, ZP>>(&ta, nullptr, &tout, p,
+                                                                                          q.stream);
+      });
+    if (t == 64) return launch_gemm_w4<W4Cfg<A::KIND, 64, typename A::WT, ZP>>(ta, tw, tout, p, q.stream);
+    if (t == 128) return launch_gemm_w4<W4Cfg<A::KIND, 128, typename A::WT, ZP>>(ta, tw, tout, p, q.stream);
+    return launch_gemm_w4<W4Cfg<A::KIND, 256, typename A::WT, ZP>>(ta, tw, tout, p, q.stream);
+  });
 }
 
 }  // namespace qb

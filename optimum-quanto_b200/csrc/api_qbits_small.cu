@@ -292,19 +292,18 @@ int qbits_small_dispatch(const QbitsArgs& q, bool* handled) {
   const int route = test_override(OVR_INT4_ROUTE);
   if (route == ROUTE_INT4_GENERAL) return OK;
   cudaStream_t st = q.stream;
-  const bool bf16 = q.dtype == DT_BF16;
   const bool zp = q.shift_is_int != 0;
   const int dbg = debug_flags();
 
   if (route == ROUTE_AUTO || route == ROUTE_INT4_RING2) {
     GemvRParams rp{};
     GemvRPlan rpl{};
-    const bool coef_aligned = reinterpret_cast<uintptr_t>(q.scale) % 16 == 0 && reinterpret_cast<uintptr_t>(q.shift) % 16 == 0;
+    const bool coef_aligned = aligned16(q.scale) && aligned16(q.shift);
     const int64_t r_groups = n / 16;
     const int r_grid = static_cast<int>(r_groups < current_sm_count() ? (r_groups > 0 ? r_groups : 1) : current_sm_count());
-    bool out_aligned = reinterpret_cast<uintptr_t>(q.out) % 16 == 0 && q.ld % 8 == 0 && q.col0 % 8 == 0;
-    for (int pq = 1; pq < q.g.n_out; ++pq) out_aligned = out_aligned && reinterpret_cast<uintptr_t>(q.g.out_peer[pq]) % 16 == 0;
-    if (out_aligned && reinterpret_cast<uintptr_t>(q.a) % 16 == 0 &&
+    bool out_aligned = aligned16(q.out) && q.ld % 8 == 0 && q.col0 % 8 == 0;
+    for (int pq = 1; pq < q.g.n_out; ++pq) out_aligned = out_aligned && aligned16(q.g.out_peer[pq]);
+    if (out_aligned && aligned16(q.a) &&
         make_gemvr_plan(m, n, k, q.group, zp, coef_aligned, r_grid, &rp, &rpl)) {
       rp.wq = q.packed;
       rp.scale = q.scale;
@@ -322,12 +321,9 @@ int qbits_small_dispatch(const QbitsArgs& q, bool* handled) {
       const int grid = r_grid;
       set_kernel_family(3);
       *handled = true;
-      if (bf16) {
-        if (zp) return launch_gemvr<__nv_bfloat16, true>(rp, rpl, grid, st);
-        return launch_gemvr<__nv_bfloat16, false>(rp, rpl, grid, st);
-      }
-      if (zp) return launch_gemvr<__half, true>(rp, rpl, grid, st);
-      return launch_gemvr<__half, false>(rp, rpl, grid, st);
+      return dispatch_act16_zp(q.dtype, q.shift_is_int, [&](auto act, auto ZP) {
+        return launch_gemvr<typename decltype(act)::WT, ZP>(rp, rpl, grid, st);
+      });
     }
     if (route == ROUTE_INT4_RING2) return fail(ERR_UNSUPPORTED, "qbits_mm: the second-generation ring gemv does not take this problem");
   }
@@ -335,8 +331,8 @@ int qbits_small_dispatch(const QbitsArgs& q, bool* handled) {
   if (route == ROUTE_AUTO || route == ROUTE_INT4_RING) {
     GemvSParams gp{};
     int smem_bytes = 0;
-    const bool coef_aligned = reinterpret_cast<uintptr_t>(q.scale) % 16 == 0 && reinterpret_cast<uintptr_t>(q.shift) % 16 == 0;
-    if (reinterpret_cast<uintptr_t>(q.a) % 16 == 0 && make_gemvs_plan(m, n, k, q.group, zp, coef_aligned, &gp, &smem_bytes)) {
+    const bool coef_aligned = aligned16(q.scale) && aligned16(q.shift);
+    if (aligned16(q.a) && make_gemvs_plan(m, n, k, q.group, zp, coef_aligned, &gp, &smem_bytes)) {
       gp.wq = q.packed;
       gp.scale = q.scale;
       gp.shift = q.shift;
@@ -359,17 +355,17 @@ int qbits_small_dispatch(const QbitsArgs& q, bool* handled) {
       const int grid = static_cast<int>(half_n < current_sm_count() ? half_n : current_sm_count());
       set_kernel_family(3);
       *handled = true;
-      if (bf16) {
-        if (zp) return launch_gemvs<__nv_bfloat16, true>(gp, grid, smem_bytes, st);
 #ifdef QB_DEVELOPER_KNOCKOUTS
+      // the knock-out variants exist for bf16 with a float shift only
+      if (q.dtype == DT_BF16 && !zp) {
         if ((dbg & 3) == 1) return launch_gemvs<__nv_bfloat16, false, 1>(gp, grid, smem_bytes, st);
         if ((dbg & 3) == 2) return launch_gemvs<__nv_bfloat16, false, 2>(gp, grid, smem_bytes, st);
         if ((dbg & 3) == 3) return launch_gemvs<__nv_bfloat16, false, 3>(gp, grid, smem_bytes, st);
-#endif
-        return launch_gemvs<__nv_bfloat16, false>(gp, grid, smem_bytes, st);
       }
-      if (zp) return launch_gemvs<__half, true>(gp, grid, smem_bytes, st);
-      return launch_gemvs<__half, false>(gp, grid, smem_bytes, st);
+#endif
+      return dispatch_act16_zp(q.dtype, q.shift_is_int, [&](auto act, auto ZP) {
+        return launch_gemvs<typename decltype(act)::WT, ZP>(gp, grid, smem_bytes, st);
+      });
     }
     if (route == ROUTE_INT4_RING) return fail(ERR_UNSUPPORTED, "qbits_mm: the ring gemv does not take this problem");
   }
@@ -408,13 +404,9 @@ int qbits_small_dispatch(const QbitsArgs& q, bool* handled) {
   d.dbg = dbg;
   *handled = true;
   set_kernel_family(3);
-  const int mi = static_cast<int>(m);
-  if (bf16) {
-    if (zp) return launch_gemv_mt<__nv_bfloat16, true>(mi, q.packed, q.a, d, pl.grid, st);
-    return launch_gemv_mt<__nv_bfloat16, false>(mi, q.packed, q.a, d, pl.grid, st);
-  }
-  if (zp) return launch_gemv_mt<__half, true>(mi, q.packed, q.a, d, pl.grid, st);
-  return launch_gemv_mt<__half, false>(mi, q.packed, q.a, d, pl.grid, st);
+  return dispatch_act16_zp(q.dtype, q.shift_is_int, [&](auto act, auto ZP) {
+    return launch_gemv_mt<typename decltype(act)::WT, ZP>(static_cast<int>(m), q.packed, q.a, d, pl.grid, st);
+  });
 }
 
 }  // namespace qb

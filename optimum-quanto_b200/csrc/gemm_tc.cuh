@@ -21,6 +21,7 @@
 
 #include "common.cuh"
 #include "gather.cuh"
+#include "host_common.cuh"
 #include "quantize_math.cuh"
 #include "wgmma_pipe.cuh"
 
@@ -1106,6 +1107,38 @@ __global__ void __launch_bounds__(Cfg::NTHREADS, 1)
 
   __syncthreads();
   if (threadIdx.x == 0) gather_signal_end(p.g);  // fused all-gather: publish "this rank's slab has landed everywhere"
+}
+
+// ------------------------------------------------------------------------------------------------
+// Host side
+// ------------------------------------------------------------------------------------------------
+// Parameters of a problem with one dense [M, N] output of `out_dt` elements (g.n_out = 1, ld = N, col0 = 0); every
+// other field zero.
+inline GemmParams dense_gemm_params(void* out, const void* bias, int out_dt, int64_t m, int64_t n, int64_t k) {
+  GemmParams p{};
+  p.bias = bias;
+  p.out = out;
+  p.g.out_peer[0] = out;
+  p.g.n_out = 1;
+  p.g.world = 1;
+  p.ld = static_cast<int>(n);
+  p.col0 = 0;
+  p.out_dt = out_dt;
+  p.M = static_cast<int>(m);
+  p.N = static_cast<int>(n);
+  p.K = static_cast<int>(k);
+  return p;
+}
+
+// Launch gemm_tc_kernel<Cfg> over p's tiles.  A null tensor map is passed zeroed: the operand the kernel's own warps
+// stage (the weights of INT4 / BYTES, both operands of F8) and the output of every epilogue but the int4 TMA store.
+template <class Cfg>
+int launch_gemm_tc(const CUtensorMap* ta, const CUtensorMap* tb, const CUtensorMap* tout, const GemmParams& p,
+                   cudaStream_t stream, const char* what = "gemm_tc_kernel launch") {
+  const CUtensorMap zero{};
+  return launch_persistent<gemm_tc_kernel<Cfg>, typename Cfg::Pipe>(p.num_m_blocks * p.num_n_blocks, stream, what,
+                                                                    ta ? *ta : zero, tb ? *tb : zero,
+                                                                    tout ? *tout : zero, p);
 }
 
 }  // namespace qb

@@ -1,10 +1,12 @@
 // Host-side plumbing shared by the translation units that hold the extern "C" entry points: status reporting,
 // per-DEVICE caches (SM count, architecture check, dynamic shared-memory opt-in), the persistent-kernel launch, TMA
-// descriptor encoding and the test hooks that pick among equivalent kernels.
+// descriptor encoding, the mapping of run-time dtype codes to kernel template arguments and the test hooks that pick
+// among equivalent kernels.
 #pragma once
 
 #include <atomic>
 #include <cstdint>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -81,9 +83,62 @@ int make_tmap_packed(CUtensorMap* map, const uint8_t* packed, int64_t rows, int6
 // box_rows rows of one batch, 128-byte swizzle.  A box never crosses a batch: past `rows` TMA fills zeros.
 int make_tmap_3d_bytes(CUtensorMap* map, const void* base, int64_t batch, int64_t rows, int64_t cols,
                        int64_t batch_stride, int box_rows);
-// [rows, cols] view with an explicit row pitch and box: the epilogue's TMA stores into (a column slab of) the output.
-int make_tmap_2d_view(CUtensorMap* map, const void* base, int dt, int64_t rows, int64_t cols, int64_t pitch_elems,
-                      int box_cols, int box_rows, bool swizzle128);
+
+// TMA operands, vector loads and bulk copies need 16-byte aligned addresses
+inline bool aligned16(const void* ptr) { return reinterpret_cast<uintptr_t>(ptr) % 16 == 0; }
+
+// ---- run-time codes -> template arguments.  Each dispatch_* helper calls the generic lambda `f` with a tag type for the
+// code it is given, so that `f` names the kernel configuration once and instantiates it for exactly the codes listed
+// here.  The entry points validate their arguments first: a code outside a helper's set is a dispatch bug, reported as
+// ERR_ARG rather than run as some other type.
+
+// 16-bit activation dtype: the staged element type and the MMA kind that consumes it
+template <typename WT_, MmaKind KIND_>
+struct Act16 {
+  using WT = WT_;
+  static constexpr MmaKind KIND = KIND_;
+};
+
+// DT_BF16 / DT_F16 -> Act16<__nv_bfloat16, BF16> / Act16<__half, F16>
+template <class F>
+int dispatch_act16(int dtype, F&& f) {
+  if (dtype == DT_BF16) return f(Act16<__nv_bfloat16, MmaKind::BF16>{});
+  if (dtype == DT_F16) return f(Act16<__half, MmaKind::F16>{});
+  return fail(ERR_ARG, "dispatch: activation dtype %d is neither bf16 nor fp16", dtype);
+}
+
+// shift_is_int -> std::bool_constant ZP: the int4 shift is an integer zero-point (else a float shift)
+template <class F>
+int dispatch_zp(int shift_is_int, F&& f) {
+  if (shift_is_int != 0) return f(std::true_type{});
+  return f(std::false_type{});
+}
+
+// the dtype x zero-point pair of the int4 kernels: f(Act16 tag, bool_constant ZP)
+template <class F>
+int dispatch_act16_zp(int dtype, int shift_is_int, F&& f) {
+  return dispatch_act16(dtype, [&](auto act) { return dispatch_zp(shift_is_int, [&](auto zp) { return f(act, zp); }); });
+}
+
+// 8-bit weight dtype -> std::integral_constant WKIND: 0 int8, 1 float8_e4m3fn, 2 float8_e5m2, 3 float8_e4m3fnuz
+template <class F>
+int dispatch_wkind(int w_dtype, F&& f) {
+  switch (w_dtype) {
+    case DT_I8: return f(std::integral_constant<int, 0>{});
+    case DT_E4M3: return f(std::integral_constant<int, 1>{});
+    case DT_E5M2: return f(std::integral_constant<int, 2>{});
+    case DT_E4M3FNUZ: return f(std::integral_constant<int, 3>{});
+    default: return fail(ERR_ARG, "dispatch: weight dtype %d is not an 8-bit type", w_dtype);
+  }
+}
+
+// rows per wgmma tile 64 / 128 -> std::integral_constant MWG (consumer warpgroups) 1 / 2
+template <class F>
+int dispatch_mwg(int tile_m, F&& f) {
+  if (tile_m == 64) return f(std::integral_constant<int, 1>{});
+  if (tile_m == 128) return f(std::integral_constant<int, 2>{});
+  return fail(ERR_ARG, "dispatch: tile height %d is neither 64 nor 128", tile_m);
+}
 
 // ---- test hooks (include/quanto_b200.h: qb200_test_override).  Every value selects a kernel that computes the same
 // result; 0 = automatic choice.  They exist so that the test-suite can execute every shipped instantiation.

@@ -238,22 +238,23 @@ def test_fnuz_qlinear_golden(golden_dir):
 # K % 128 != 0 for int8 x int8 (TMA), K % 64 == 32 with groups of 32 for int4.
 def _census():
     rows = []
-    # api_qbits.cu:28-36 launch_int4<MWG>: bf16/f16 x float shift / zero-point, MWG 1 / 2 (api_qbits.cu:100-101)
+    # api_qbits.cu GemmCfg<KIND, BSrc::INT4, MWG, 128, WT, ZP>: bf16/f16 x float shift / zero-point, MWG 1 / 2
     for tag in ("bf16", "f16"):
         for zp in (False, True):
             for tm in (64, 128):
                 rows.append((f"int4-{tag}-{'zp' if zp else 'shift'}-m{tm}", "int4", zp, tm, 128,
                              65 if tm == 64 else 129, 336, 352, tag))
-    # api_qbytes.cu:124-125 launch_int8<MWG, BN>
+    # api_qbytes.cu GemmCfg<MmaKind::I8, BSrc::TMA, MWG, BN>
     for j, (tm, bn) in enumerate(((64, 128), (64, 256), (128, 128), (128, 256))):
         rows.append((f"int8-m{tm}-n{bn}", "int8", None, tm, bn, 65 if tm == 64 else 200, 301, 592,
                      ("bf16", "f16", "f32", "bf16")[j]))
-    # api_qbytes.cu:40-49 launch_fp8<MWG>: (activation, weight) pairs, MWG 1 / 2 (api_qbytes.cu:115-116)
+    # api_qbytes.cu F8Cfg<MWG, WKIND, AKIND>: (activation, weight) pairs, MWG 1 / 2
     for j, (ak, wk) in enumerate((("e4m3fn", "e4m3fn"), ("e5m2", "e4m3fn"), ("e4m3fn", "e5m2"), ("e5m2", "e5m2"))):
         for tm in (64, 128):
             rows.append((f"fp8-{ak}-{wk}-m{tm}", "fp8", (ak, wk), tm, 128, 65 if tm == 64 else 129, 301,
                          (528, 544, 560)[(2 * j + tm // 128) % 3], ("bf16", "f16")[j % 2]))
-    # api_qbytes.cu:148-161 QB_LAUNCH_BYTES: bf16/f16 activations x int8/e4m3fn/e5m2/e4m3fnuz weights, MWG 2 / 1
+    # api_qbytes.cu GemmCfg<KIND, BSrc::BYTES, MWG, 128, WT, false, WKIND>: bf16/f16 activations x
+    # int8/e4m3fn/e5m2/e4m3fnuz weights, MWG 2 / 1
     for tag in ("bf16", "f16"):
         for j, wk in enumerate(("int8", "e4m3fn", "e5m2", "e4m3fnuz")):
             for tm in (64, 128):
