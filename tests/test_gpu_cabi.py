@@ -204,16 +204,22 @@ def test_qbits_mm_gemv_ring(tag, M, N, K, G):
     shift_t = torch.from_numpy(shift).cuda() if zeropoint else bits_to_torch(shift, tag)
     args = (bits_to_torch(x_bits, tag), torch.from_numpy(packed).cuda(), bits_to_torch(scale, tag), shift_t,
             None if bias_bits is None else bits_to_torch(bias_bits, tag), N, K, G)
-    lib = native().load()
-    y1 = cabi_qbits_mm(*args)
-    fam = lib.qb200_last_kernel_family()
-    y2 = cabi_qbits_mm(*args, use_workspace=False)  # the ring kernel needs no workspace
-    torch.cuda.synchronize()
+    n = native()
+    lib = n.load()
+    # forced: the automatic route sends the Llama-sized shapes here to the second-generation kernel instead
+    with n.test_override(n.OVR_INT4_ROUTE, n.ROUTE_INT4_RING):
+        y1 = cabi_qbits_mm(*args)
+        fam = lib.qb200_last_kernel_family()
+        y2 = cabi_qbits_mm(*args, use_workspace=False)  # the ring kernel needs no workspace
+        torch.cuda.synchronize()
     assert fam == 3
     assert torch.equal(y1, y2)
     _check_linear(y1, x_bits, deq_bits, bias_bits, tag, ("gemv_ring", tag, M, N, K, G))
+    y0 = cabi_qbits_mm(*args)  # the dispatcher's own choice passes the same bound
+    torch.cuda.synchronize()
+    _check_linear(y0, x_bits, deq_bits, bias_bits, tag, ("auto", tag, M, N, K, G))
     if K % 128 == 0:  # the stream-K warp-MMA kernel this one replaced for M <= 8 (still the 8 < M <= 32 candidate)
-        with native().test_override(native().OVR_INT4_ROUTE, native().ROUTE_INT4_GEMV):
+        with n.test_override(n.OVR_INT4_ROUTE, n.ROUTE_INT4_GEMV):
             y3 = cabi_qbits_mm(*args)
             torch.cuda.synchronize()
         _check_linear(y3, x_bits, deq_bits, bias_bits, tag, ("streamk", tag, M, N, K, G))
