@@ -184,6 +184,25 @@ QB200_API int64_t qb200_qbytes_bmm_workspace_bytes(int64_t batch, int64_t n, int
 QB200_API int qb200_qbytes_softmax(const void* x, const void* scale, const void* out_scale, void* out, int64_t rows,
                                    int64_t cols, int q_dtype, int scale_dtype, void* stream);
 
+/* ---- quantized layer norm (the reference's QLayerNorm, optimum/quanto/nn/qlayernorm.py:27-53) -------------------- */
+
+/* F.layer_norm over rows of h elements (qlayernorm.py:52-53), optionally from and to 8-bit codes, in one launch
+ * (family 6).  Replaces F.layer_norm after qfallback's dequantize of an ActivationQBytesTensor input
+ * (tensor/qbytes.py:23-31) followed by the quantize_output hook (nn/qmodule.py:296-302 -> library/quantize.py:51-55):
+ *   x   = x[r, i] in `dtype`, or rnd_dt(in_scale * payload) when in_dtype is a code dtype
+ *   y   = rnd_dt(weight[i] * (x - mean) / sqrt(var + eps) + bias[i])   fp32 mean, then the biased variance about it;
+ *                                                                        1 / sqrt correctly rounded
+ *   out = y in `dtype` (out_dtype == dtype), or quantize_symmetric(y, out_dtype, out_scale): the quotient y / out_scale
+ *         rounded to `dtype`, then rint / clamp / cast as qb200_quantize_symmetric.
+ * x: dense [rows, h] of in_dtype, in `dtype` in {F32, F16, BF16} or codes in {I8, E4M3, E5M2, E4M3FNUZ}; in_scale: ONE
+ * element of `dtype` (codes in only).  weight, bias: [h] in `dtype`, each may be NULL.  out: dense [rows, h] of
+ * out_dtype (`dtype` or a code dtype).  out_scale: ONE element of out_scale_dtype in {F32, dtype}, read on the device
+ * (codes out only; F32 with a 16-bit dtype divides by the fp32 value, as ATen's CPU division by a 0-dim fp32 tensor
+ * does).  Any h >= 1; rows of up to 16384 elements are read from memory once. */
+QB200_API int qb200_layer_norm(const void* x, const void* in_scale, const void* weight, const void* bias,
+                               const void* out_scale, void* out, int64_t rows, int64_t h, double eps, int in_dtype,
+                               int dtype, int out_dtype, int out_scale_dtype, void* stream);
+
 /* ---- quantized 2-D convolution (the reference's QConv2d, optimum/quanto/nn/qconv2d.py) -------------------------- */
 
 /* out = F.conv2d(x, dequantize(W), bias, stride, padding, dilation) with groups == 1, as an implicit GEMM on the tensor
@@ -298,10 +317,11 @@ QB200_API int64_t qb200_quantize_qbits_hqq_workspace_bytes(int64_t n, int64_t k,
 QB200_API int qb200_hqq_shrink(const void* x, void* out, int64_t numel, double beta, double lp_norm, int dtype,
                                void* stream);
 
-/* Which kernel family the last qb200_qbytes_mm / qb200_qbytes_bmm / qb200_qbits_mm / *_grad_input call on this thread dispatched to:
+/* Which kernel family the last qb200_qbytes_mm / qb200_qbytes_bmm / qb200_qbits_mm / *_grad_input / qb200_layer_norm call on this thread dispatched to:
  * 0 none, 1 wgmma (TMA + warpgroup MMA), 2 CUDA-core (shape-agnostic), 3 warp-MMA gemv (int4, M <= 32: TMA ring or register streaming),
  * 4 byte-transpose pass + wgmma (qb200_qbytes_bmm with a B that is not K-contiguous), 5 implicit-GEMM convolution
- * (qb200_qbits_conv2d / qb200_qbytes_conv2d).
+ * (qb200_qbits_conv2d / qb200_qbytes_conv2d), 6 layer norm (qb200_layer_norm: one warp per row up to 1024 elements, one
+ * CTA per row above).
  * For tests and bench accounting. */
 QB200_API int qb200_last_kernel_family(void);
 

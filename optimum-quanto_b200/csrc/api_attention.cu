@@ -225,14 +225,6 @@ static int qbytes_bmm_impl(const void* a, const void* b, const void* sa, const v
 constexpr int kSmThreads = 128;
 constexpr int kSmCache = 32768;
 
-template <int Q>
-__device__ __forceinline__ float decode8(uint32_t v) {
-  if constexpr (Q == DT_I8) return static_cast<float>(static_cast<int8_t>(static_cast<uint8_t>(v)));
-  else if constexpr (Q == DT_E4M3) return e4m3_to_float(static_cast<uint8_t>(v));
-  else if constexpr (Q == DT_E5M2) return e5m2_to_float(static_cast<uint8_t>(v));
-  else return e4m3fnuz_to_float(static_cast<uint8_t>(v));
-}
-
 // (m, s) <- the running (max, sum) of the union of two sets of values
 __device__ __forceinline__ void softmax_merge(float& m, float& s, float m2, float s2) {
   if (s2 == 0.f) return;

@@ -85,6 +85,15 @@ __device__ __forceinline__ uint8_t quantize_one(float t) {
   }
 }
 
+// the payload of an 8-bit code of dtype Q (the low byte of v) as a float: the int8 value or the fp8 value
+template <int Q>
+__device__ __forceinline__ float decode8(uint32_t v) {
+  if constexpr (Q == DT_I8) return static_cast<float>(static_cast<int8_t>(static_cast<uint8_t>(v)));
+  else if constexpr (Q == DT_E4M3) return e4m3_to_float(static_cast<uint8_t>(v));
+  else if constexpr (Q == DT_E5M2) return e5m2_to_float(static_cast<uint8_t>(v));
+  else return e4m3fnuz_to_float(static_cast<uint8_t>(v));
+}
+
 // quanto::quantize_affine for one element (optimum/quanto/library/quantize.py:71-78), arithmetic in dtype T:
 //   float shift : clamp(rint(rnd(rnd(b + z) / s)), 0, qmax)
 //   zero-point  : clamp(rnd(rint(rnd(b / s)) + zp), 0, qmax)

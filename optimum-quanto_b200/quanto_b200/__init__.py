@@ -7,6 +7,7 @@ its absence is an error (no CPU / eager fallback).
 from . import library  # noqa: F401  (op registration side effect)
 from . import library_attention  # noqa: F401  (quantized attention ops)
 from . import library_conv  # noqa: F401  (quantized conv2d ops)
+from . import library_norm  # noqa: F401  (quantized layer norm op)
 from .calibrate import *  # noqa: F401,F403
 from .nn import *  # noqa: F401,F403
 from .pipeline import *  # noqa: F401,F403

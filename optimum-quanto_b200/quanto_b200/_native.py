@@ -63,6 +63,7 @@ EXPORTS = (
     "qb200_qbytes_softmax",
     "qb200_qbits_conv2d",
     "qb200_qbytes_conv2d",
+    "qb200_layer_norm",
 )
 
 # qb200_test_override keys (include/quanto_b200.h)
@@ -156,6 +157,7 @@ def load():
         lib.qb200_qbytes_softmax.argtypes = [vp, vp, vp, vp, i64, i64, i32, i32, vp]
         lib.qb200_qbits_conv2d.argtypes = [vp, vp, vp, vp, vp, vp] + [i64] * 7 + [i32] * 10 + [vp]
         lib.qb200_qbytes_conv2d.argtypes = [vp, vp, vp, vp, vp] + [i64] * 7 + [i32] * 8 + [vp]
+        lib.qb200_layer_norm.argtypes = [vp, vp, vp, vp, vp, vp, i64, i64, f64, i32, i32, i32, i32, vp]
         for name in EXPORTS:
             getattr(lib, name)  # AttributeError here == header and library out of sync
         # Developer knock-outs exist only in a `make KNOCKOUTS=1` build and are set explicitly through

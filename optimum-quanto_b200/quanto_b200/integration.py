@@ -33,10 +33,14 @@ After this, every `optimum.quanto` object keeps working as before -- `quantize()
    runs `quanto::qbits_conv2d` / `quanto::qbytes_conv2d` -- one implicit-GEMM launch -- when no graph is needed and the
    kernel takes the problem, instead of qfallback's dense dequantised copy + cuDNN; everything else keeps the
    reference's route.
+8. the reference's `QLayerNorm` (optimum/quanto/nn/qlayernorm.py) runs `quanto::qbytes_layer_norm` -- the layer norm
+   and its output quantisation in one launch, from floats or codes -- under the conditions of the package's QLayerNorm
+   (library_norm.qlayernorm_forward), except while a `Calibration` mode is active; its quantize_output hook passes the
+   op's codes through instead of quantizing them again.
 
 Used by tools/run_reference_tests.py to run the reference's OWN hot-path tests (tests/library, tests/tensor/ops,
 tests/nn/test_qlinear.py, and for 6 tests/tensor/ops/test_mm_dispatch.py, tests/tensor/activations/test_activations_dispatch.py,
-tests/nn/test_qattention.py, for 7 tests/nn/test_qconv2d.py) against these kernels.  Nothing here is imported by the rest of the package.
+tests/nn/test_qattention.py, for 7 tests/nn/test_qconv2d.py, for 8 tests/nn/test_qlayernorm.py) against these kernels.  Nothing here is imported by the rest of the package.
 """
 import torch
 
@@ -210,4 +214,35 @@ def bind_reference():
 
     RefQBits.__torch_function__ = conv_torch_function(RefQBits.__torch_function__.__func__)
     RefQBytesW.__torch_function__ = conv_torch_function(RefQBytesW.__torch_function__.__func__)
+
+    # ---- 8. QLayerNorm: the layer norm and its output quantisation in one launch (library_norm.qlayernorm_forward)
+    from optimum.quanto.calibrate import Calibration as RefCalibration
+    from optimum.quanto.nn import qmodule as ref_qmodule
+    from optimum.quanto.nn.qlayernorm import QLayerNorm as RefQLayerNorm
+
+    from . import library_norm
+
+    orig_ln_forward = RefQLayerNorm.forward
+
+    def ln_forward(self, input):
+        # calibrate_output must see the float output: keep the composition while a Calibration mode is active
+        if not any(isinstance(m, RefCalibration) for m in torch.overrides._get_current_function_mode_stack()):
+            # the reference's disable_output_quantization removes the hook but keeps its handle
+            handle = self._quantize_hooks.get("output")
+            live = handle is not None and handle.id in self._forward_hooks
+            out = library_norm.qlayernorm_forward(self, input, RefActivation, live)
+            if out is not None:
+                return out
+        return orig_ln_forward(self, input)
+
+    RefQLayerNorm.forward = ln_forward
+    orig_quantize_activation = ref_qmodule.quantize_activation
+
+    def quantize_activation(t, qtype, scale):
+        # the quantize_output hook of a QLayerNorm that returned the op's codes with this very scale: nothing to do
+        if isinstance(t, RefActivation) and t.qtype == qtype and t._scale is scale:
+            return t
+        return orig_quantize_activation(t, qtype=qtype, scale=scale)
+
+    ref_qmodule.quantize_activation = quantize_activation
     _bound = True

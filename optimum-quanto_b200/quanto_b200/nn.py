@@ -1,9 +1,11 @@
-"""Quantized `torch.nn.Linear` and `torch.nn.Conv2d` (the callers of the hot path).
+"""Quantized `torch.nn.Linear`, `torch.nn.Conv2d` and `torch.nn.LayerNorm` (the callers of the hot path).
 
 `QLinear.forward` is `F.linear(input, self.qweight, bias)` exactly as optimum/quanto/nn/qlinear.py:49-50; the
 weight's `__torch_function__` turns that into one `quanto::qbytes_mm` or `quanto::qbits_mm` launch.  `QConv2d.forward`
 is `self._conv_forward(input, self.qweight, self.bias)` as optimum/quanto/nn/qconv2d.py; F.conv2d on a frozen weight
 becomes one `quanto::qbits_conv2d` / `quanto::qbytes_conv2d` launch where the kernel takes the problem.
+`QLayerNorm` (optimum/quanto/nn/qlayernorm.py) runs F.layer_norm and its output quantisation as one
+`quanto::qbytes_layer_norm` launch when no gradient is needed (library_norm.qlayernorm_forward).
 `QModuleMixin` keeps the reference's constructor arguments, hooks, state-dict keys and freeze semantics
 (optimum/quanto/nn/qmodule.py:94-312).
 """
@@ -12,11 +14,12 @@ from typing import Optional, Union
 import torch
 
 from . import _native
+from .library_norm import qlayernorm_forward
 from .tensor import (AbsmaxOptimizer, ActivationQBytesTensor, HqqOptimizer, MaxOptimizer, Optimizer, QTensor,
                      SymmetricOptimizer, PackedTensor, WeightQBitsTensor, WeightQBytesTensor, qint2, qint4, qtype, qtypes,
                      quantize_activation, quantize_weight)
 
-__all__ = ["QModuleMixin", "QLinear", "QConv2d", "freeze"]
+__all__ = ["QModuleMixin", "QLinear", "QConv2d", "QLayerNorm", "freeze"]
 
 
 def _pick_group_size(in_features: int) -> Optional[int]:
@@ -270,6 +273,26 @@ class QConv2d(QModuleMixin, torch.nn.Conv2d):
     def forward(self, input: torch.Tensor) -> torch.Tensor:
         # a padding_mode other than 'zeros' pads with F.pad here, then the conv itself runs with padding 0
         return self._conv_forward(input, self.qweight, self.bias)
+
+
+class QLayerNorm(QModuleMixin, torch.nn.LayerNorm):
+    """optimum/quanto/nn/qlayernorm.py: created only with `activations` set; the weight and bias are never quantized and
+    the output is quantized per tensor with `output_scale`."""
+
+    @classmethod
+    def qcreate(cls, module, weights: Optional[qtype] = None, activations: Optional[qtype] = None,
+                optimizer: Optional[Optimizer] = None, device: Optional[torch.device] = None):
+        if activations is None:
+            return None
+        dtype = None if module.weight is None else module.weight.dtype
+        return cls(module.normalized_shape, module.eps, module.elementwise_affine, module.bias is not None, dtype=dtype,
+                   device=device, weights=None, activations=activations, optimizer=None)
+
+    def forward(self, input: torch.Tensor) -> torch.Tensor:
+        out = qlayernorm_forward(self, input, ActivationQBytesTensor, "output" in self._quantize_hooks)
+        if out is not None:
+            return out
+        return torch.nn.functional.layer_norm(input, self.normalized_shape, self.weight, self.bias, self.eps)
 
 
 def freeze(model: torch.nn.Module):

@@ -9,7 +9,7 @@ Selected tests (reference paths): tests/library/test_unpack.py, test_quantize.py
 tests/tensor/test_packed_tensor.py, tests/tensor/ops/test_linear_dispatch.py, tests/tensor/weights (canonical classes),
 tests/tensor/optimizers/test_hqq_optimizer.py, tests/nn/test_qlinear.py, and the quantized-attention tests
 tests/tensor/ops/test_mm_dispatch.py, tests/tensor/activations/test_activations_dispatch.py, tests/nn/test_qattention.py,
-and the quantized convolution tests tests/nn/test_qconv2d.py.
+the quantized convolution tests tests/nn/test_qconv2d.py and the quantized layer norm tests tests/nn/test_qlayernorm.py.
 The tests of the retired AWQ / Marlin / TinyGemm
 bindings are deselected (those ops are no longer reached; INTEGRATION.md)."""
 import os
@@ -34,7 +34,7 @@ def main():
            "tensor/weights/test_weight_qbytes_tensor_dispatch.py", "tensor/weights/test_weight_qbytes_tensor_quantize.py",
            "tensor/optimizers/test_hqq_optimizer.py", "nn/test_qlinear.py",
            "tensor/ops/test_mm_dispatch.py", "tensor/activations/test_activations_dispatch.py", "nn/test_qattention.py",
-           "nn/test_qconv2d.py"]
+           "nn/test_qconv2d.py", "nn/test_qlayernorm.py"]
     extra = [a for a in sys.argv[1:] if a != "--cpu"]
     cmd = [sys.executable, "-m", "pytest", "-q", "-p", "quanto_b200_bind", "-x" if "--cpu" in sys.argv else "--maxfail=50",
            "--deselect", "nn/test_qlinear.py::test_qlinear_gradient"] + sel + extra
