@@ -288,6 +288,17 @@ QB200_API int qb200_quantize_qbits_max(const void* base, uint8_t* packed, void* 
  * by this call (running maximum + CTA ticket; the last CTA publishes the result). */
 QB200_API int qb200_absmax(const void* base, void* out, void* scratch, int64_t numel, int dtype, void* stream);
 
+/* One calibration step of a per-tensor activation scale, in place and without a host synchronisation: absmax_scale
+ * (optimum/quanto/calibrate.py:37-61) and the momentum update of Calibration (calibrate.py:31-34) as ONE launch.
+ *   new    = rnd(max|base| / qmax)                  true division, rounded to `dtype`
+ *   *scale = (*scale == 1) ? new : rnd(rnd(*scale * m) + rnd(new * om)),  m = (float)momentum, om = (float)(1 - momentum)
+ * Every rnd rounds to `dtype`, as the reference's ATen ops do; a NaN in base gives a NaN scale.  base: `numel` >= 1
+ * elements of `dtype` (f32 / f16 / bf16), any alignment (16-byte aligned bases take vector loads); scale: one element
+ * of `dtype`; `scratch`: 8 bytes of device memory, 4-byte aligned, zeroed on the stream by this call.  QB200_ERR_ARG
+ * for an empty tensor, a non-float dtype, qmax <= 0 or a misaligned scratch buffer. */
+QB200_API int qb200_absmax_update(const void* base, void* scale, void* scratch, int64_t numel, int dtype, double qmax,
+                                  double momentum, void* stream);
+
 /* freeze() of an axis-0 8-bit weight in ONE launch: AbsmaxOptimizer (optimum/quanto/tensor/optimizers/
  * absmax_optimizer.py:29-36: scale[n] = max|W[n,:]| / qmax, qmax = 127 / 448 / 57344) + quanto::quantize_symmetric
  * (optimum/quanto/library/quantize.py:51-55).  base [n, k] `dtype`; out [n, k] out_dtype in {I8, E4M3, E5M2};

@@ -6,6 +6,7 @@
 //                                 + quantize_affine + pack_weights for an axis-0 grouped weight as ONE launch:
 //                                 reads the float weight once (2 B/weight), writes 0.5 B/weight + scale/shift
 //   absmax                     -- calibrate.py:37-61 absmax_scale, per-tensor reduction
+//   absmax_update              -- absmax_scale + the Calibration scale update (calibrate.py:31-34), in place, one launch
 //   quantize_qbytes_absmax     -- AbsmaxOptimizer (tensor/optimizers/absmax_optimizer.py:29-36) + quantize_symmetric
 //                                 (library/quantize.py:51-55) for an axis-0 8-bit weight as ONE launch
 //
@@ -428,10 +429,10 @@ __device__ __forceinline__ float block_max_256(float m, float* red) {
   return r;
 }
 
+// One thread's max |base[i]| over its grid-stride share: 16-byte vector loads when `vec_ok` (base 16-byte aligned) with
+// a scalar tail, scalar loads otherwise.
 template <typename T>
-__global__ void __launch_bounds__(kFzThreads)
-    absmax_kernel(const T* __restrict__ base, T* __restrict__ out, int* __restrict__ scratch, int64_t numel, int vec_ok) {
-  __shared__ float red[kFzThreads / 32];
+__device__ __forceinline__ float thread_absmax(const T* __restrict__ base, int64_t numel, int vec_ok) {
   const int64_t tid = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
   float m = 0.f;
@@ -455,18 +456,51 @@ __global__ void __launch_bounds__(kFzThreads)
   } else {
     for (int64_t i = tid; i < numel; i += stride) m = nanmax(m, fabsf(to_float<T>(base[i])));
   }
-  m = block_max_256(m, red);
-  if (threadIdx.x == 0) {
-    // scratch[0] = running maximum (bit pattern of a non-negative float; a NaN's pattern is the largest of all, so the
-    // integer atomicMax propagates it), scratch[1] = CTAs done; the last CTA
-    // publishes the result in T, so the caller needs no conversion launch
-    atomicMax(scratch, __float_as_int(m));
-    __threadfence();
-    const int done = atomicAdd(scratch + 1, 1);
-    if (done == static_cast<int>(gridDim.x) - 1) {
-      __threadfence();
-      out[0] = from_float<T>(__int_as_float(atomicMax(scratch, 0)));
-    }
+  return m;
+}
+
+// Thread 0 of each CTA folds the CTA's maximum `m` into scratch[0] (bit pattern of a non-negative float; a NaN's
+// pattern is the largest of all, so the integer atomicMax propagates it) and takes a ticket from scratch[1].  Returns
+// true in the last CTA only, with *total = the maximum over the whole grid.
+__device__ __forceinline__ bool publish_absmax(float m, int* __restrict__ scratch, float* total) {
+  atomicMax(scratch, __float_as_int(m));
+  __threadfence();
+  const int done = atomicAdd(scratch + 1, 1);
+  if (done != static_cast<int>(gridDim.x) - 1) return false;
+  __threadfence();
+  *total = __int_as_float(atomicMax(scratch, 0));
+  return true;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kFzThreads)
+    absmax_kernel(const T* __restrict__ base, T* __restrict__ out, int* __restrict__ scratch, int64_t numel, int vec_ok) {
+  __shared__ float red[kFzThreads / 32];
+  const float m = block_max_256(thread_absmax<T>(base, numel, vec_ok), red);
+  float total;
+  // the last CTA publishes the result in T, so the caller needs no conversion launch
+  if (threadIdx.x == 0 && publish_absmax(m, scratch, &total)) out[0] = from_float<T>(total);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// absmax_update: one calibration step of a per-tensor scale, in place (optimum/quanto/calibrate.py:31-34 with
+// absmax_scale, :37-61).  The last CTA evaluates, each rounding to T where the reference's ATen ops round:
+//   new   = rnd(max / qmax)                                         (true division, as absmax_scale)
+//   scale = scale == 1 ? new : rnd(rnd(scale * m) + rnd(new * om))  (m = float(momentum), om = float(1 - momentum))
+// The `scale == 1` test is read here on the device: the reference's torch.all(scale == 1) is a host synchronisation.
+// ---------------------------------------------------------------------------------------------------------------
+template <typename T>
+__global__ void __launch_bounds__(kFzThreads)
+    absmax_update_kernel(const T* __restrict__ base, T* __restrict__ scale, int* __restrict__ scratch, int64_t numel,
+                         int vec_ok, float qmax, float m, float om) {
+  __shared__ float red[kFzThreads / 32];
+  const float bm = block_max_256(thread_absmax<T>(base, numel, vec_ok), red);
+  float total;
+  if (threadIdx.x == 0 && publish_absmax(bm, scratch, &total)) {
+    const float fresh = rnd<T>(__fdiv_rn(total, qmax));
+    const float old = to_float<T>(scale[0]);
+    const float upd = old == 1.f ? fresh : rnd<T>(__fadd_rn(rnd<T>(__fmul_rn(old, m)), rnd<T>(__fmul_rn(fresh, om))));
+    scale[0] = from_float<T>(upd);
   }
 }
 
@@ -624,6 +658,30 @@ int qb200_absmax(const void* base, void* out, void* scratch, int64_t numel, int 
     default: return set_error(ERR_ARG, "absmax: dtype %d not floating point", dtype);
   }
   return cudaGetLastError() == cudaSuccess ? OK : set_error(ERR_CUDA, "absmax: launch failed");
+}
+
+int qb200_absmax_update(const void* base, void* scale, void* scratch, int64_t numel, int dtype, double qmax,
+                        double momentum, void* stream) {
+  if (numel < 1) return set_error(ERR_ARG, "absmax_update: the tensor is empty (numel %lld)", (long long)numel);
+  if (!base || !scale || !scratch) return set_error(ERR_ARG, "absmax_update: null buffer");
+  if (reinterpret_cast<uintptr_t>(scratch) % 4 != 0)
+    return set_error(ERR_ARG, "absmax_update: scratch must be 4-byte aligned");
+  if (!(qmax > 0.0)) return set_error(ERR_ARG, "absmax_update: qmax must be positive");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int vec_ok = reinterpret_cast<uintptr_t>(base) % 16 == 0;
+  const int grid = fz_grid((numel + 15) / 16, 8);
+  int* sc = static_cast<int*>(scratch);
+  // the python scalars become float operands of ATen's float opmath: momentum, and 1 - momentum evaluated in double
+  const float q = static_cast<float>(qmax), m = static_cast<float>(momentum), om = static_cast<float>(1.0 - momentum);
+  if (dtype != DT_F32 && dtype != DT_F16 && dtype != DT_BF16)
+    return set_error(ERR_ARG, "absmax_update: dtype %d not floating point", dtype);
+  if (cudaMemsetAsync(scratch, 0, 8, st) != cudaSuccess) return set_error(ERR_CUDA, "absmax_update: memset failed");
+  switch (dtype) {
+    case DT_F32: absmax_update_kernel<float><<<grid, kFzThreads, 0, st>>>(static_cast<const float*>(base), static_cast<float*>(scale), sc, numel, vec_ok, q, m, om); break;
+    case DT_F16: absmax_update_kernel<__half><<<grid, kFzThreads, 0, st>>>(static_cast<const __half*>(base), static_cast<__half*>(scale), sc, numel, vec_ok, q, m, om); break;
+    default: absmax_update_kernel<__nv_bfloat16><<<grid, kFzThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(base), static_cast<__nv_bfloat16*>(scale), sc, numel, vec_ok, q, m, om); break;
+  }
+  return cudaGetLastError() == cudaSuccess ? OK : set_error(ERR_CUDA, "absmax_update: launch failed");
 }
 
 int qb200_quantize_qbytes_absmax(const void* base, void* out, void* scale, int64_t n, int64_t k, int dtype,

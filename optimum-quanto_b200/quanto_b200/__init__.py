@@ -8,9 +8,11 @@ from . import library  # noqa: F401  (op registration side effect)
 from . import library_attention  # noqa: F401  (quantized attention ops)
 from . import library_conv  # noqa: F401  (quantized conv2d ops)
 from . import library_norm  # noqa: F401  (quantized layer norm op)
+from . import library_calibrate  # noqa: F401  (in-place calibration scale update op)
 from .calibrate import *  # noqa: F401,F403
 from .nn import *  # noqa: F401,F403
 from .pipeline import *  # noqa: F401,F403
+from .quantize import *  # noqa: F401,F403
 from .tensor import *  # noqa: F401,F403
 
 __version__ = "0.1.0"

@@ -64,6 +64,7 @@ EXPORTS = (
     "qb200_qbits_conv2d",
     "qb200_qbytes_conv2d",
     "qb200_layer_norm",
+    "qb200_absmax_update",
 )
 
 # qb200_test_override keys (include/quanto_b200.h)
@@ -158,6 +159,7 @@ def load():
         lib.qb200_qbits_conv2d.argtypes = [vp, vp, vp, vp, vp, vp] + [i64] * 7 + [i32] * 10 + [vp]
         lib.qb200_qbytes_conv2d.argtypes = [vp, vp, vp, vp, vp] + [i64] * 7 + [i32] * 8 + [vp]
         lib.qb200_layer_norm.argtypes = [vp, vp, vp, vp, vp, vp, i64, i64, f64, i32, i32, i32, i32, vp]
+        lib.qb200_absmax_update.argtypes = [vp, vp, vp, i64, i32, f64, f64, vp]
         for name in EXPORTS:
             getattr(lib, name)  # AttributeError here == header and library out of sync
         # Developer knock-outs exist only in a `make KNOCKOUTS=1` build and are set explicitly through

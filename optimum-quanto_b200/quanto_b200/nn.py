@@ -14,6 +14,7 @@ from typing import Optional, Union
 import torch
 
 from . import _native
+from .calibrate import calibrating
 from .library_norm import qlayernorm_forward
 from .tensor import (AbsmaxOptimizer, ActivationQBytesTensor, HqqOptimizer, MaxOptimizer, Optimizer, QTensor,
                      SymmetricOptimizer, PackedTensor, WeightQBitsTensor, WeightQBytesTensor, qint2, qint4, qtype, qtypes,
@@ -245,12 +246,13 @@ class QLinear(QModuleMixin, torch.nn.Linear):
         """Quantized activations in AND out with a frozen 8-bit weight: the linear, its bias and the `quantize_output`
         hook (nn/qmodule.py:300-302) as ONE `quanto::qbytes_linear_quantized` launch (SURVEY 8f rank 2) -- the [M, N]
         result is never written in 16 bits and read back.  Bit-identical to `F.linear` followed by the hook; inference
-        only (no graph).  Returns None when the ordinary path has to run."""
+        only (no graph).  Returns None when the ordinary path has to run, and while a `Calibration` mode needs to
+        see the float output."""
         w = self.weight
         if ("output" not in self._quantize_hooks or not isinstance(input, ActivationQBytesTensor)
                 or not isinstance(w, WeightQBytesTensor) or not w._data.is_cuda or w.axis != 0 or w.ndim != 2
                 or input._data.dtype != self.activation_qtype.dtype
-                or (torch.is_grad_enabled() and (input.requires_grad or w.requires_grad))):
+                or (torch.is_grad_enabled() and (input.requires_grad or w.requires_grad)) or calibrating()):
             return None
         scales = input._scale * w._scale  # in the module dtype, one rounding (tensor/weights/qbytes.py:72-73)
         data = torch.ops.quanto.qbytes_linear_quantized(input._data, w._data, scales, self.bias, self.output_scale,
@@ -289,9 +291,10 @@ class QLayerNorm(QModuleMixin, torch.nn.LayerNorm):
                    device=device, weights=None, activations=activations, optimizer=None)
 
     def forward(self, input: torch.Tensor) -> torch.Tensor:
-        out = qlayernorm_forward(self, input, ActivationQBytesTensor, "output" in self._quantize_hooks)
-        if out is not None:
-            return out
+        if not calibrating():  # the output calibration has to see F.layer_norm's float output
+            out = qlayernorm_forward(self, input, ActivationQBytesTensor, "output" in self._quantize_hooks)
+            if out is not None:
+                return out
         return torch.nn.functional.layer_norm(input, self.normalized_shape, self.weight, self.bias, self.eps)
 
 
