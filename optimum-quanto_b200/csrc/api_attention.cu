@@ -130,30 +130,18 @@ static int64_t bmm_copy_bytes(int64_t batch, int64_t n, int64_t k, int64_t b_bs)
   return (b_bs == 0 ? 1 : batch) * n * k;
 }
 
-template <typename T>
-static int launch_bmm_simt(const void* a, const void* b, const void* sa, const void* sb, int dt, void* out, int64_t batch,
-                           int64_t m, int64_t n, int64_t k, int64_t a_bs, int64_t b_bs, int b_layout, cudaStream_t st) {
-  const int64_t b_sk = b_layout == 0 ? 1 : n, b_sn = b_layout == 0 ? k : 1;
-  dim3 grid(static_cast<unsigned>((n + kST - 1) / kST), static_cast<unsigned>((m + kST - 1) / kST),
-            static_cast<unsigned>(batch));
-  qbytes_bmm_simt_kernel<T><<<grid, 256, 0, st>>>(static_cast<const int8_t*>(a), static_cast<const int8_t*>(b), sa, sb, dt,
-                                                  static_cast<T*>(out), static_cast<int>(m), static_cast<int>(n),
-                                                  static_cast<int>(k), a_bs, b_bs, b_sk, b_sn);
-  return check_cuda(cudaGetLastError(), "qbytes_bmm CUDA-core launch");
-}
-
 static int qbytes_bmm_impl(const void* a, const void* b, const void* sa, const void* sb, void* out, void* ws,
                            int64_t ws_bytes, int64_t batch, int64_t m, int64_t n, int64_t k, int64_t a_bs, int64_t b_bs,
                            int b_layout, int dt, cudaStream_t st) {
   set_kernel_family(0);
   if (batch < 0 || m < 0 || n < 0 || k <= 0 || a_bs < 0 || b_bs < 0) return fail(ERR_ARG, "qbytes_bmm: bad shape");
   if (b_layout != 0 && b_layout != 1) return fail(ERR_ARG, "qbytes_bmm: b_layout must be 0 (K-contiguous) or 1 (N-contiguous)");
-  if (dt != DT_F32 && dt != DT_F16 && dt != DT_BF16) return fail(ERR_ARG, "qbytes_bmm: scale dtype must be floating point");
+  if (!is_float_dtype(dt)) return fail(ERR_ARG, "qbytes_bmm: scale dtype must be floating point");
   if (sa == nullptr || sb == nullptr) return fail(ERR_ARG, "qbytes_bmm: scales missing");
   if (m > INT32_MAX || n > INT32_MAX || k > INT32_MAX || batch > INT32_MAX)
     return fail(ERR_UNSUPPORTED, "qbytes_bmm: dimension too large");
   if (batch == 0 || m == 0 || n == 0) return OK;
-  int rc = check_arch();
+  int rc = check_arch("qbytes_bmm");
   if (rc != OK) return rc;
   const int route = test_override(OVR_BMM_ROUTE);
   const bool copy = bmm_needs_copy(b_layout);
@@ -208,9 +196,16 @@ static int qbytes_bmm_impl(const void* a, const void* b, const void* sa, const v
   if (batch > 65535 || (m + kST - 1) / kST > 65535)
     return fail(ERR_UNSUPPORTED, "qbytes_bmm: the CUDA-core kernel takes at most 65535 batches of 65535 x 64 rows");
   set_kernel_family(2);
-  if (dt == DT_BF16) return launch_bmm_simt<__nv_bfloat16>(a, b, sa, sb, dt, out, batch, m, n, k, a_bs, b_bs, b_layout, st);
-  if (dt == DT_F16) return launch_bmm_simt<__half>(a, b, sa, sb, dt, out, batch, m, n, k, a_bs, b_bs, b_layout, st);
-  return launch_bmm_simt<float>(a, b, sa, sb, dt, out, batch, m, n, k, a_bs, b_bs, b_layout, st);
+  const int64_t b_sk = b_layout == 0 ? 1 : n, b_sn = b_layout == 0 ? k : 1;
+  dim3 grid(static_cast<unsigned>((n + kST - 1) / kST), static_cast<unsigned>((m + kST - 1) / kST),
+            static_cast<unsigned>(batch));
+  return dispatch_float(dt, [&](auto out_dt) {
+    using T = typename decltype(out_dt)::T;
+    qbytes_bmm_simt_kernel<T><<<grid, 256, 0, st>>>(static_cast<const int8_t*>(a), static_cast<const int8_t*>(b), sa, sb,
+                                                    dt, static_cast<T*>(out), static_cast<int>(m), static_cast<int>(n),
+                                                    static_cast<int>(k), a_bs, b_bs, b_sk, b_sn);
+    return check_cuda(cudaGetLastError(), "qbytes_bmm CUDA-core launch");
+  });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -316,21 +311,6 @@ __global__ void __launch_bounds__(kSmThreads)
   }
 }
 
-template <typename T>
-static int launch_softmax_t(const void* x, const void* scale, const void* out_scale, void* out, int64_t rows,
-                            int64_t cols, int q_dt, cudaStream_t st) {
-  const unsigned grid = static_cast<unsigned>(rows < (1 << 20) ? rows : (1 << 20));
-  const auto* xp = static_cast<const uint8_t*>(x);
-  const auto* sp = static_cast<const T*>(scale);
-  const auto* op = static_cast<const T*>(out_scale);
-  auto* o = static_cast<uint8_t*>(out);
-  if (q_dt == DT_I8) qbytes_softmax_kernel<T, DT_I8><<<grid, kSmThreads, 0, st>>>(xp, sp, op, o, rows, cols);
-  else if (q_dt == DT_E4M3) qbytes_softmax_kernel<T, DT_E4M3><<<grid, kSmThreads, 0, st>>>(xp, sp, op, o, rows, cols);
-  else if (q_dt == DT_E5M2) qbytes_softmax_kernel<T, DT_E5M2><<<grid, kSmThreads, 0, st>>>(xp, sp, op, o, rows, cols);
-  else qbytes_softmax_kernel<T, DT_E4M3FNUZ><<<grid, kSmThreads, 0, st>>>(xp, sp, op, o, rows, cols);
-  return check_cuda(cudaGetLastError(), "qbytes_softmax launch");
-}
-
 }  // namespace qb
 
 using namespace qb;
@@ -352,17 +332,23 @@ int qb200_qbytes_bmm(const void* a, const void* b, const void* scale_a, const vo
 int qb200_qbytes_softmax(const void* x, const void* scale, const void* out_scale, void* out, int64_t rows, int64_t cols,
                          int q_dtype, int scale_dtype, void* stream) {
   if (rows < 0 || cols <= 0) return fail(ERR_ARG, "qbytes_softmax: bad shape");
-  if (q_dtype != DT_I8 && q_dtype != DT_E4M3 && q_dtype != DT_E5M2 && q_dtype != DT_E4M3FNUZ)
-    return fail(ERR_ARG, "qbytes_softmax: unsupported code dtype %d", q_dtype);
+  if (!is_code_dtype(q_dtype)) return fail(ERR_ARG, "qbytes_softmax: unsupported code dtype %d", q_dtype);
   if (scale == nullptr || out_scale == nullptr) return fail(ERR_ARG, "qbytes_softmax: scales missing");
   if (rows == 0) return OK;
-  int rc = check_arch();
+  if (!is_float_dtype(scale_dtype)) return fail(ERR_ARG, "qbytes_softmax: scale dtype must be floating point");
+  int rc = check_arch("qbytes_softmax");
   if (rc != OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (scale_dtype == DT_BF16) return launch_softmax_t<__nv_bfloat16>(x, scale, out_scale, out, rows, cols, q_dtype, st);
-  if (scale_dtype == DT_F16) return launch_softmax_t<__half>(x, scale, out_scale, out, rows, cols, q_dtype, st);
-  if (scale_dtype == DT_F32) return launch_softmax_t<float>(x, scale, out_scale, out, rows, cols, q_dtype, st);
-  return fail(ERR_ARG, "qbytes_softmax: scale dtype must be floating point");
+  const unsigned grid = static_cast<unsigned>(rows < (1 << 20) ? rows : (1 << 20));
+  return dispatch_float(scale_dtype, [&](auto dt) {
+    return dispatch_code8(q_dtype, [&](auto Q) {
+      using T = typename decltype(dt)::T;
+      qbytes_softmax_kernel<T, Q><<<grid, kSmThreads, 0, st>>>(static_cast<const uint8_t*>(x), static_cast<const T*>(scale),
+                                                               static_cast<const T*>(out_scale),
+                                                               static_cast<uint8_t*>(out), rows, cols);
+      return check_cuda(cudaGetLastError(), "qbytes_softmax launch");
+    });
+  });
 }
 
 }  // extern "C"

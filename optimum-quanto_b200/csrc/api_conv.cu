@@ -86,7 +86,7 @@ int qb200_qbits_conv2d(const void* x, const uint8_t* packed, const void* scale, 
     return fail(ERR_UNSUPPORTED, "qbits_conv2d: group %d is neither a multiple of 32 nor K", group);
   if (!aligned16(packed)) return fail(ERR_UNSUPPORTED, "qbits_conv2d: packed weights not 16-byte aligned");
   if (p.M == 0) return OK;
-  rc = check_arch();
+  rc = check_arch("qbits_conv2d");
   if (rc != OK) return rc;
   p.wq = packed;
   p.wscale = scale;
@@ -108,8 +108,7 @@ int qb200_qbytes_conv2d(const void* x, const void* wq, const void* scales, const
                         int64_t cin, int64_t h, int64_t w, int64_t cout, int64_t kh, int64_t kw, int stride_h,
                         int stride_w, int pad_h, int pad_w, int dil_h, int dil_w, int w_dtype, int dtype, void* stream) {
   set_kernel_family(0);
-  if (w_dtype != DT_I8 && w_dtype != DT_E4M3 && w_dtype != DT_E5M2 && w_dtype != DT_E4M3FNUZ)
-    return fail(ERR_ARG, "qbytes_conv2d: weights must be int8 or float8");
+  if (!is_code_dtype(w_dtype)) return fail(ERR_ARG, "qbytes_conv2d: weights must be int8 or float8");
   const ConvArgs a{x, bias, out, batch, cin, h, w, cout, kh, kw, stride_h, stride_w, pad_h, pad_w, dil_h, dil_w, dtype,
                    static_cast<cudaStream_t>(stream)};
   GemmParams p;
@@ -118,7 +117,7 @@ int qb200_qbytes_conv2d(const void* x, const void* wq, const void* scales, const
   if (rc != OK) return rc;
   if (!aligned16(wq)) return fail(ERR_UNSUPPORTED, "qbytes_conv2d: weights not 16-byte aligned");
   if (p.M == 0) return OK;
-  rc = check_arch();
+  rc = check_arch("qbytes_conv2d");
   if (rc != OK) return rc;
   p.wq = static_cast<const uint8_t*>(wq);
   p.wscale = scales;

@@ -1,5 +1,5 @@
-// extern "C" entry points that are not GEMMs (include/quanto_b200.h) and the host-side state every translation unit
-// shares: last-error text, per-device caches, TMA descriptor encoding, test hooks, developer flags.
+// The host-side state every translation unit shares (last-error text, per-device caches, TMA descriptor encoding, test
+// hooks, developer flags) and the extern "C" entry points that query or set it (include/quanto_b200.h).
 #include "../../include/quanto_b200.h"
 
 #include <cstdarg>
@@ -11,11 +11,6 @@
 
 namespace qb {
 
-int launch_unpack(const uint8_t*, uint8_t*, int64_t, int, cudaStream_t);
-int launch_quantize_symmetric(const void*, const void*, void*, int64_t, int64_t, int, int, int, cudaStream_t);
-int launch_dequantize_qbits(const uint8_t*, const void*, const void*, void*, int64_t, int64_t, int, int, int, int,
-                            cudaStream_t);
-
 static thread_local char g_err[512] = "";
 static thread_local int g_family = 0;
 static std::atomic<int> g_override[OVR_COUNT];
@@ -25,15 +20,6 @@ static std::atomic<long long*> g_trace{nullptr};
 #endif
 
 int fail(int code, const char* fmt, ...) {
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(g_err, sizeof(g_err), fmt, ap);
-  va_end(ap);
-  return code;
-}
-
-// same as fail(): the entry points that live next to their kernels (freeze.cu) report through this name
-int set_error(int code, const char* fmt, ...) {
   va_list ap;
   va_start(ap, fmt);
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
@@ -94,16 +80,18 @@ int current_sm_count() {
   return sms;
 }
 
-int check_arch() {
-  const int dev = current_device();
-  if (dev < 0) return fail(ERR_CUDA, "no CUDA device");
+int check_arch(const char* what) {
+  int dev = -1;
+  const cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return fail(ERR_CUDA, "%s: no current CUDA device: %s", what, cudaGetErrorString(e));
   int major = (dev < kMaxDevices) ? g_dev[dev].cc_major.load(std::memory_order_relaxed) : -1;
   if (major < 0) {
     major = 0;
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
     if (dev < kMaxDevices) g_dev[dev].cc_major.store(major, std::memory_order_relaxed);
   }
-  return major == 9 ? OK : fail(ERR_ARCH, "quanto_b200 kernels are built for sm_90a only (device %d is sm_%d)", dev, major);
+  if (major == 9) return OK;
+  return fail(ERR_ARCH, "%s: quanto_b200 kernels are built for sm_90a only (device %d is sm_%d)", what, dev, major);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -241,33 +229,6 @@ int qb200_developer_build(void) {
 #else
   return 0;
 #endif
-}
-
-int qb200_unpack(const uint8_t* in, uint8_t* out, int64_t n_bytes, int bits, void* stream) {
-  if (bits != 2 && bits != 4) return fail(ERR_ARG, "unpack: bits must be 2 or 4, got %d", bits);
-  if (n_bytes < 0 || (n_bytes > 0 && (in == nullptr || out == nullptr))) return fail(ERR_ARG, "unpack: bad buffer");
-  int rc = launch_unpack(in, out, n_bytes, bits, static_cast<cudaStream_t>(stream));
-  return rc == OK ? OK : fail(rc, "unpack: launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-}
-
-int qb200_quantize_symmetric(const void* base, const void* scale, void* out, int64_t outer, int64_t inner,
-                             int axis_mode, int in_dtype, int out_dtype, void* stream) {
-  if (in_dtype != DT_F32 && in_dtype != DT_F16 && in_dtype != DT_BF16)
-    return fail(ERR_ARG, "quantize_symmetric: input dtype %d not floating point", in_dtype);
-  if (out_dtype != DT_I8 && out_dtype != DT_E4M3 && out_dtype != DT_E5M2 && out_dtype != DT_E4M3FNUZ)
-    return fail(ERR_ARG, "quantize_symmetric: unsupported target dtype %d", out_dtype);
-  if (axis_mode < 0 || axis_mode > 2) return fail(ERR_ARG, "quantize_symmetric: axis_mode %d", axis_mode);
-  int rc = launch_quantize_symmetric(base, scale, out, outer, inner, axis_mode, in_dtype, out_dtype,
-                                     static_cast<cudaStream_t>(stream));
-  return rc == OK ? OK : fail(rc, "quantize_symmetric: launch failed");
-}
-
-int qb200_dequantize_qbits(const uint8_t* packed, const void* scale, const void* shift, void* out, int64_t n,
-                           int64_t k, int group, int bits, int dtype, int shift_is_int, void* stream) {
-  int rc = launch_dequantize_qbits(packed, scale, shift, out, n, k, group, bits, dtype, shift_is_int,
-                                   static_cast<cudaStream_t>(stream));
-  return rc == OK ? OK : fail(rc, "dequantize_qbits: invalid arguments or launch failure (N=%lld K=%lld group=%d bits=%d)",
-                              (long long)n, (long long)k, group, bits);
 }
 
 }  // extern "C"

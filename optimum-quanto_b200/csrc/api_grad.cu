@@ -23,8 +23,7 @@ static int qbits_grad_input_impl(const void* grad_out, const uint8_t* packed, co
                                  cudaStream_t stream) {
   set_kernel_family(0);
   if (m < 0 || n <= 0 || k <= 0 || group <= 0) return fail(ERR_ARG, "qbits_mm_grad_input: bad shape");
-  if (dtype != DT_BF16 && dtype != DT_F16 && dtype != DT_F32)
-    return fail(ERR_ARG, "qbits_mm_grad_input: dtype must be f32, f16 or bf16");
+  if (!is_float_dtype(dtype)) return fail(ERR_ARG, "qbits_mm_grad_input: dtype must be f32, f16 or bf16");
   if (k % group != 0) return fail(ERR_ARG, "qbits_mm_grad_input: group %d does not divide K = %lld", group, (long long)k);
   if (m > INT32_MAX || n > INT32_MAX || k > INT32_MAX) return fail(ERR_UNSUPPORTED, "qbits_mm_grad_input: dimension too large");
   if (dtype == DT_F32) return fail(ERR_UNSUPPORTED, "qbits_mm_grad_input: the kernel takes f16 / bf16 gradients");
@@ -33,7 +32,7 @@ static int qbits_grad_input_impl(const void* grad_out, const uint8_t* packed, co
   if (!aligned16(grad_out) || !aligned16(packed) || !aligned16(grad_in))
     return fail(ERR_UNSUPPORTED, "qbits_mm_grad_input: grad_out, packed and grad_in must be 16-byte aligned");
   if (m == 0) return OK;
-  int rc = check_arch();
+  int rc = check_arch("qbits_mm_grad_input");
   if (rc == OK) rc = make_context_current();
   if (rc != OK) return rc;
 
@@ -66,17 +65,15 @@ static int qbytes_grad_input_impl(const void* grad_out, const void* w, const voi
                                   int64_t n, int64_t k, int w_dtype, int dtype, cudaStream_t stream) {
   set_kernel_family(0);
   if (m < 0 || n <= 0 || k <= 0) return fail(ERR_ARG, "qbytes_mm_grad_input: bad shape");
-  if (w_dtype != DT_I8 && w_dtype != DT_E4M3 && w_dtype != DT_E5M2 && w_dtype != DT_E4M3FNUZ)
-    return fail(ERR_ARG, "qbytes_mm_grad_input: weights must be int8 or float8");
-  if (dtype != DT_BF16 && dtype != DT_F16 && dtype != DT_F32)
-    return fail(ERR_ARG, "qbytes_mm_grad_input: dtype must be f32, f16 or bf16");
+  if (!is_code_dtype(w_dtype)) return fail(ERR_ARG, "qbytes_mm_grad_input: weights must be int8 or float8");
+  if (!is_float_dtype(dtype)) return fail(ERR_ARG, "qbytes_mm_grad_input: dtype must be f32, f16 or bf16");
   if (m > INT32_MAX || n > INT32_MAX || k > INT32_MAX) return fail(ERR_UNSUPPORTED, "qbytes_mm_grad_input: dimension too large");
   if (dtype == DT_F32) return fail(ERR_UNSUPPORTED, "qbytes_mm_grad_input: the kernel takes f16 / bf16 gradients");
   if (n % 8 != 0 || k % 16 != 0) return fail(ERR_UNSUPPORTED, "qbytes_mm_grad_input: needs N %% 8 == 0 and K %% 16 == 0");
   if (!aligned16(grad_out) || !aligned16(w) || !aligned16(grad_in))
     return fail(ERR_UNSUPPORTED, "qbytes_mm_grad_input: grad_out, w and grad_in must be 16-byte aligned");
   if (m == 0) return OK;
-  int rc = check_arch();
+  int rc = check_arch("qbytes_mm_grad_input");
   if (rc == OK) rc = make_context_current();
   if (rc != OK) return rc;
 

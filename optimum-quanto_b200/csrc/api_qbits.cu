@@ -53,12 +53,12 @@ static int qbits_mm_impl(QbitsArgs& q) {
   const int64_t m = q.m, n = q.n, k = q.k;
   const int group = q.group, dtype = q.dtype;
   if (m < 0 || n <= 0 || k <= 0 || group <= 0) return fail(ERR_ARG, "qbits_mm: bad shape");
-  if (dtype != DT_BF16 && dtype != DT_F16 && dtype != DT_F32) return fail(ERR_ARG, "qbits_mm: dtype must be f32, f16 or bf16");
+  if (!is_float_dtype(dtype)) return fail(ERR_ARG, "qbits_mm: dtype must be f32, f16 or bf16");
   if (q.bits != 4 && q.bits != 2) return fail(ERR_ARG, "qbits_mm: bits must be 2 or 4 (got %d)", q.bits);
   if (k % group != 0) return fail(ERR_ARG, "qbits_mm: group %d does not divide K = %lld", group, (long long)k);
   if (m > INT32_MAX || n > INT32_MAX || k > INT32_MAX || q.ld > INT32_MAX) return fail(ERR_UNSUPPORTED, "qbits_mm: dimension too large");
   if (m == 0) return OK;
-  int rc = check_arch();
+  int rc = check_arch("qbits_mm");
   if (rc != OK) return rc;
   const bool gathered = q.g.n_out > 1;
   // tensor-core kernels: 4-bit, 16-bit activations, N even, K % 16 == 0, group 32 or a multiple of 64, aligned buffers.
@@ -68,9 +68,8 @@ static int qbits_mm_impl(QbitsArgs& q) {
   if (!tc_ok) {
     if (gathered) return fail(ERR_UNSUPPORTED, "qbits_mm_gather: the fused gather exists for the tensor-core kernels only");
     set_kernel_family(2);
-    rc = launch_qbits_mm_simt(q.a, q.packed, q.scale, q.shift, q.bias, q.out, static_cast<int>(m), static_cast<int>(n),
-                              static_cast<int>(k), group, q.bits, dtype, q.shift_is_int, q.ld, q.col0, q.stream);
-    return rc == OK ? OK : fail(rc, "qbits_mm: CUDA-core kernel launch failed");
+    return launch_qbits_mm_simt(q.a, q.packed, q.scale, q.shift, q.bias, q.out, static_cast<int>(m), static_cast<int>(n),
+                                static_cast<int>(k), group, q.bits, dtype, q.shift_is_int, q.ld, q.col0, q.stream);
   }
   q.group_log2 = group_log2(group);
 

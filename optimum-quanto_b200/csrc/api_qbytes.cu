@@ -31,14 +31,12 @@ static int qbytes_mm_impl(const void* a, const void* w, const void* scales, cons
                           void* stream) {
   set_kernel_family(0);
   if (m < 0 || n <= 0 || k <= 0) return fail(ERR_ARG, "qbytes_mm: bad shape");
-  if (out_dtype != DT_F32 && out_dtype != DT_F16 && out_dtype != DT_BF16)
-    return fail(ERR_ARG, "qbytes_mm: scales/out dtype must be floating point");
-  if (w_dtype != DT_I8 && w_dtype != DT_E4M3 && w_dtype != DT_E5M2 && w_dtype != DT_E4M3FNUZ)
-    return fail(ERR_ARG, "qbytes_mm: weights must be int8 or float8");
+  if (!is_float_dtype(out_dtype)) return fail(ERR_ARG, "qbytes_mm: scales/out dtype must be floating point");
+  if (!is_code_dtype(w_dtype)) return fail(ERR_ARG, "qbytes_mm: weights must be int8 or float8");
   if (a_dtype < DT_F32 || a_dtype > DT_E4M3FNUZ || a_dtype == DT_U8) return fail(ERR_ARG, "qbytes_mm: bad activation dtype");
   if (m > INT32_MAX || n > INT32_MAX || k > INT32_MAX) return fail(ERR_UNSUPPORTED, "qbytes_mm: dimension too large");
   if (m == 0) return OK;
-  int rc = check_arch();
+  int rc = check_arch("qbytes_mm");
   if (rc != OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int route = test_override(OVR_QBYTES_ROUTE);
@@ -115,9 +113,8 @@ static int qbytes_mm_impl(const void* a, const void* w, const void* scales, cons
     });
   }
   set_kernel_family(2);
-  rc = launch_qbytes_mm_simt(a, w, scales, bias, out, static_cast<int>(m), static_cast<int>(n), static_cast<int>(k),
-                             a_dtype, w_dtype, out_dtype, st);
-  return rc == OK ? OK : fail(rc, "qbytes_mm: CUDA-core kernel launch failed");
+  return launch_qbytes_mm_simt(a, w, scales, bias, out, static_cast<int>(m), static_cast<int>(n), static_cast<int>(k),
+                               a_dtype, w_dtype, out_dtype, st);
 }
 
 }  // namespace qb
@@ -134,7 +131,8 @@ int qb200_qbytes_mm(const void* a, const void* w, const void* scales, const void
 int qb200_qbytes_mm_quantized(const void* a, const void* w, const void* scales, const void* bias, void* out_q,
                               const void* out_scale, int64_t m, int64_t n, int64_t k, int a_dtype, int w_dtype,
                               int scale_dtype, int q_dtype, void* stream) {
-  if (q_dtype != DT_I8 && q_dtype != DT_E4M3 && q_dtype != DT_E5M2)
+  // no float8_e4m3fnuz output: the fused epilogue quantises to int8, e4m3fn and e5m2 only
+  if (!is_code_dtype(q_dtype) || q_dtype == DT_E4M3FNUZ)
     return fail(ERR_ARG, "qbytes_mm_quantized: unsupported target dtype %d", q_dtype);
   if (scales == nullptr || out_scale == nullptr) return fail(ERR_ARG, "qbytes_mm_quantized: scales / out_scale missing");
   return qbytes_mm_impl(a, w, scales, bias, out_q, m, n, k, a_dtype, w_dtype, scale_dtype, q_dtype, out_scale, stream);

@@ -3,22 +3,15 @@
 //   quantize_symmetric -- replaces the 3-4 ATen launches of optimum/quanto/library/quantize.py:51-55
 //   dequantize_qbits   -- QBitsDequantizer.forward, optimum/quanto/tensor/qbits.py:27-49, as ONE launch
 // All are 128-bit vectorised, grid-stride, launched on the caller's stream.
-#include <type_traits>
+#include "../../include/quanto_b200.h"
 
-#include "common.cuh"
+#include "host_common.cuh"
 #include "quantize_math.cuh"
 
 namespace qb {
 
 constexpr int kEwThreads = 256;
-
-static inline int ew_grid(int64_t work_items) {
-  int64_t blocks = (work_items + kEwThreads - 1) / kEwThreads;
-  int64_t cap = static_cast<int64_t>(kNumSMsH100) * 16;  // 16 resident CTAs of 256 threads cover 2048 thr/SM x2 waves
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return static_cast<int>(blocks);
-}
+constexpr int kEwCtasPerSm = 16;  // 16 resident CTAs of 256 threads cover 2048 thr/SM x2 waves
 
 // ---------------------------------------------------------------------------------------------
 // unpack: out[p * n + i] = (in[i] >> (bits * p)) & mask        (planes concatenated along dim 0)
@@ -54,31 +47,6 @@ __global__ void __launch_bounds__(kEwThreads) unpack_scalar_kernel(const uint8_t
 #pragma unroll
     for (int p = 0; p < PLANES; ++p) out[static_cast<int64_t>(p) * n + i] = static_cast<uint8_t>((v >> (BITS * p)) & MASK);
   }
-}
-
-int launch_unpack(const uint8_t* in, uint8_t* out, int64_t n_bytes, int bits, cudaStream_t stream) {
-  if (bits != 2 && bits != 4) return ERR_ARG;
-  if (n_bytes < 0) return ERR_ARG;
-  if (n_bytes == 0) return OK;
-  const bool vec = (n_bytes % 16 == 0) && (reinterpret_cast<uintptr_t>(in) % 16 == 0) &&
-                   (reinterpret_cast<uintptr_t>(out) % 16 == 0);
-  if (vec) {
-    const int64_t n_vec = n_bytes / 16;
-    const int grid = ew_grid(n_vec);
-    if (bits == 4)
-      unpack_vec_kernel<4><<<grid, kEwThreads, 0, stream>>>(reinterpret_cast<const uint4*>(in),
-                                                            reinterpret_cast<uint4*>(out), n_vec);
-    else
-      unpack_vec_kernel<2><<<grid, kEwThreads, 0, stream>>>(reinterpret_cast<const uint4*>(in),
-                                                            reinterpret_cast<uint4*>(out), n_vec);
-  } else {
-    const int grid = ew_grid(n_bytes);
-    if (bits == 4)
-      unpack_scalar_kernel<4><<<grid, kEwThreads, 0, stream>>>(in, out, n_bytes);
-    else
-      unpack_scalar_kernel<2><<<grid, kEwThreads, 0, stream>>>(in, out, n_bytes);
-  }
-  return cudaGetLastError() == cudaSuccess ? OK : ERR_CUDA;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -164,49 +132,6 @@ __global__ void __launch_bounds__(kEwThreads)
   }
 }
 
-template <typename T, int OUT_DT>
-static int launch_qs_t(const void* base, const void* scale, void* out, int64_t numel, int64_t inner, int axis_mode,
-                       cudaStream_t stream) {
-  const bool vec = (inner % 8 == 0) && (numel % 8 == 0) && (reinterpret_cast<uintptr_t>(base) % 16 == 0) &&
-                   (reinterpret_cast<uintptr_t>(out) % 8 == 0);
-  if (vec) {
-    constexpr int UNR = 4;
-    const int grid = ew_grid((numel / 8 + UNR - 1) / UNR);
-    quantize_symmetric_kernel<T, OUT_DT, 8, UNR><<<grid, kEwThreads, 0, stream>>>(
-        static_cast<const T*>(base), static_cast<const T*>(scale), static_cast<uint8_t*>(out), numel, inner, axis_mode);
-  } else {
-    const int grid = ew_grid(numel);
-    quantize_symmetric_kernel<T, OUT_DT, 1, 1><<<grid, kEwThreads, 0, stream>>>(
-        static_cast<const T*>(base), static_cast<const T*>(scale), static_cast<uint8_t*>(out), numel, inner, axis_mode);
-  }
-  return cudaGetLastError() == cudaSuccess ? OK : ERR_CUDA;
-}
-
-template <typename T>
-static int launch_qs_o(const void* base, const void* scale, void* out, int64_t numel, int64_t inner, int axis_mode,
-                       int out_dt, cudaStream_t stream) {
-  switch (out_dt) {
-    case DT_I8: return launch_qs_t<T, DT_I8>(base, scale, out, numel, inner, axis_mode, stream);
-    case DT_E4M3: return launch_qs_t<T, DT_E4M3>(base, scale, out, numel, inner, axis_mode, stream);
-    case DT_E5M2: return launch_qs_t<T, DT_E5M2>(base, scale, out, numel, inner, axis_mode, stream);
-    case DT_E4M3FNUZ: return launch_qs_t<T, DT_E4M3FNUZ>(base, scale, out, numel, inner, axis_mode, stream);
-    default: return ERR_ARG;
-  }
-}
-
-int launch_quantize_symmetric(const void* base, const void* scale, void* out, int64_t outer, int64_t inner,
-                              int axis_mode, int in_dt, int out_dt, cudaStream_t stream) {
-  if (outer < 0 || inner < 0 || axis_mode < 0 || axis_mode > 2) return ERR_ARG;
-  const int64_t numel = outer * inner;
-  if (numel == 0) return OK;
-  switch (in_dt) {
-    case DT_F32: return launch_qs_o<float>(base, scale, out, numel, inner, axis_mode, out_dt, stream);
-    case DT_F16: return launch_qs_o<__half>(base, scale, out, numel, inner, axis_mode, out_dt, stream);
-    case DT_BF16: return launch_qs_o<__nv_bfloat16>(base, scale, out, numel, inner, axis_mode, out_dt, stream);
-    default: return ERR_ARG;
-  }
-}
-
 // ---------------------------------------------------------------------------------------------
 // dequantize_qbits (axis 0): canonical storage is `packed[Rp, G]` with plane p of byte (r, c) holding
 // grouped row r + p*Rp (tensor/packed.py:45-69); grouped row R = n*(K/G)+g, and the axis-0 ungroup is a
@@ -262,36 +187,80 @@ __global__ void __launch_bounds__(kEwThreads)
   }
 }
 
-template <typename T>
-static int launch_deq_t(const uint8_t* packed, const void* scale, const void* shift, void* out, int64_t rows,
-                        int64_t packed_rows, int group, int bits, int shift_is_int, cudaStream_t stream) {
-  const int grid = ew_grid(packed_rows * group / 4);
-  if (bits == 4)
-    dequantize_qbits_kernel<T, 4><<<grid, kEwThreads, 0, stream>>>(packed, static_cast<const T*>(scale), shift,
-                                                                   static_cast<T*>(out), rows, packed_rows, group,
-                                                                   shift_is_int);
-  else
-    dequantize_qbits_kernel<T, 2><<<grid, kEwThreads, 0, stream>>>(packed, static_cast<const T*>(scale), shift,
-                                                                   static_cast<T*>(out), rows, packed_rows, group,
-                                                                   shift_is_int);
-  return cudaGetLastError() == cudaSuccess ? OK : ERR_CUDA;
+}  // namespace qb
+
+using namespace qb;
+
+extern "C" {
+
+int qb200_unpack(const uint8_t* in, uint8_t* out, int64_t n_bytes, int bits, void* stream) {
+  if (bits != 2 && bits != 4) return fail(ERR_ARG, "unpack: bits must be 2 or 4, got %d", bits);
+  if (n_bytes < 0 || (n_bytes > 0 && (in == nullptr || out == nullptr))) return fail(ERR_ARG, "unpack: bad buffer");
+  if (n_bytes == 0) return OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool vec = n_bytes % 16 == 0 && aligned16(in) && aligned16(out);
+  return dispatch_bits(bits, [&](auto BITS) {
+    if (vec)
+      unpack_vec_kernel<BITS><<<capped_grid(n_bytes / 16, kEwThreads, kEwCtasPerSm), kEwThreads, 0, st>>>(
+          reinterpret_cast<const uint4*>(in), reinterpret_cast<uint4*>(out), n_bytes / 16);
+    else
+      unpack_scalar_kernel<BITS><<<capped_grid(n_bytes, kEwThreads, kEwCtasPerSm), kEwThreads, 0, st>>>(in, out, n_bytes);
+    return check_cuda(cudaGetLastError(), "unpack launch");
+  });
 }
 
-int launch_dequantize_qbits(const uint8_t* packed, const void* scale, const void* shift, void* out, int64_t n,
-                            int64_t k, int group, int bits, int dt, int shift_is_int, cudaStream_t stream) {
-  if ((bits != 2 && bits != 4) || n <= 0 || k <= 0 || group <= 0) return ERR_ARG;
-  if ((n * k) % group != 0 || group % 4 != 0) return ERR_ARG;
-  if (reinterpret_cast<uintptr_t>(packed) % 4 != 0 || reinterpret_cast<uintptr_t>(out) % 16 != 0) return ERR_ARG;
+int qb200_quantize_symmetric(const void* base, const void* scale, void* out, int64_t outer, int64_t inner,
+                             int axis_mode, int in_dtype, int out_dtype, void* stream) {
+  if (!is_float_dtype(in_dtype)) return fail(ERR_ARG, "quantize_symmetric: input dtype %d not floating point", in_dtype);
+  if (!is_code_dtype(out_dtype)) return fail(ERR_ARG, "quantize_symmetric: unsupported target dtype %d", out_dtype);
+  if (axis_mode < 0 || axis_mode > 2) return fail(ERR_ARG, "quantize_symmetric: axis_mode %d", axis_mode);
+  if (outer < 0 || inner < 0)
+    return fail(ERR_ARG, "quantize_symmetric: negative shape (%lld x %lld)", (long long)outer, (long long)inner);
+  const int64_t numel = outer * inner;
+  if (numel == 0) return OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool vec = inner % 8 == 0 && numel % 8 == 0 && aligned16(base) && reinterpret_cast<uintptr_t>(out) % 8 == 0;
+  return dispatch_float(in_dtype, [&](auto in) {
+    return dispatch_code8(out_dtype, [&](auto OUT) {
+      using T = typename decltype(in)::T;
+      const T* b = static_cast<const T*>(base);
+      const T* s = static_cast<const T*>(scale);
+      uint8_t* o = static_cast<uint8_t*>(out);
+      if (vec) {
+        constexpr int UNR = 4;
+        quantize_symmetric_kernel<T, OUT, 8, UNR>
+            <<<capped_grid((numel / 8 + UNR - 1) / UNR, kEwThreads, kEwCtasPerSm), kEwThreads, 0, st>>>(
+                b, s, o, numel, inner, axis_mode);
+      } else {
+        quantize_symmetric_kernel<T, OUT, 1, 1><<<capped_grid(numel, kEwThreads, kEwCtasPerSm), kEwThreads, 0, st>>>(
+            b, s, o, numel, inner, axis_mode);
+      }
+      return check_cuda(cudaGetLastError(), "quantize_symmetric launch");
+    });
+  });
+}
+
+int qb200_dequantize_qbits(const uint8_t* packed, const void* scale, const void* shift, void* out, int64_t n,
+                           int64_t k, int group, int bits, int dtype, int shift_is_int, void* stream) {
+  if (bits != 2 && bits != 4) return fail(ERR_ARG, "dequantize_qbits: bits must be 2 or 4, got %d", bits);
+  if (n <= 0 || k <= 0 || group <= 0 || (n * k) % group != 0 || group % 4 != 0)
+    return fail(ERR_ARG, "dequantize_qbits: bad shape (N=%lld K=%lld group=%d)", (long long)n, (long long)k, group);
+  if (reinterpret_cast<uintptr_t>(packed) % 4 != 0 || !aligned16(out))
+    return fail(ERR_ARG, "dequantize_qbits: packed must be 4-byte and out 16-byte aligned");
+  if (!is_float_dtype(dtype)) return fail(ERR_ARG, "dequantize_qbits: dtype %d not floating point", dtype);
   const int64_t rows = n * k / group;
   const int planes = 8 / bits;
   const int64_t packed_rows = (rows + planes - 1) / planes;
-  switch (dt) {
-    case DT_F32: return launch_deq_t<float>(packed, scale, shift, out, rows, packed_rows, group, bits, shift_is_int, stream);
-    case DT_F16: return launch_deq_t<__half>(packed, scale, shift, out, rows, packed_rows, group, bits, shift_is_int, stream);
-    case DT_BF16:
-      return launch_deq_t<__nv_bfloat16>(packed, scale, shift, out, rows, packed_rows, group, bits, shift_is_int, stream);
-    default: return ERR_ARG;
-  }
+  const int grid = capped_grid(packed_rows * group / 4, kEwThreads, kEwCtasPerSm);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return dispatch_float(dtype, [&](auto dt) {
+    return dispatch_bits(bits, [&](auto BITS) {
+      using T = typename decltype(dt)::T;
+      dequantize_qbits_kernel<T, BITS><<<grid, kEwThreads, 0, st>>>(
+          packed, static_cast<const T*>(scale), shift, static_cast<T*>(out), rows, packed_rows, group, shift_is_int);
+      return check_cuda(cudaGetLastError(), "dequantize_qbits launch");
+    });
+  });
 }
 
-}  // namespace qb
+}  // extern "C"

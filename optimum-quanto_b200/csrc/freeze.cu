@@ -11,25 +11,14 @@
 //                                 (library/quantize.py:51-55) for an axis-0 8-bit weight as ONE launch
 //
 // All bit-exact with the reference's CPU arithmetic (see quantize_math.cuh); HBM-bound; launched on the caller's stream.
-#include <type_traits>
-
 #include "../../include/quanto_b200.h"
-#include "common.cuh"
+
+#include "host_common.cuh"
 #include "quantize_math.cuh"
 
 namespace qb {
 
-int set_error(int code, const char* fmt, ...);  // api.cu: records the thread's last error text, returns `code`
-
 constexpr int kFzThreads = 256;
-
-static inline int fz_grid(int64_t threads_needed, int ctas_per_sm) {
-  int64_t blocks = (threads_needed + kFzThreads - 1) / kFzThreads;
-  const int64_t cap = static_cast<int64_t>(kNumSMsH100) * ctas_per_sm;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return static_cast<int>(blocks);
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // quantize_affine (unfused): base viewed as [outer, inner] (already grouped); scale/shift index = row (axis_mode 1),
@@ -87,29 +76,6 @@ __global__ void __launch_bounds__(kFzThreads)
   }
 }
 
-template <typename T, bool ZP>
-static int launch_qa_t(const void* base, const void* scale, const void* shift, uint8_t* out, int64_t numel,
-                       int64_t inner, int axis_mode, float qmax, int zp_signed, cudaStream_t stream) {
-  const bool vec = (inner % 8 == 0) && (reinterpret_cast<uintptr_t>(base) % 16 == 0) &&
-                   (reinterpret_cast<uintptr_t>(out) % 8 == 0);
-  if (vec) {
-    quantize_affine_kernel<T, ZP, 8><<<fz_grid(numel / 8, 16), kFzThreads, 0, stream>>>(
-        static_cast<const T*>(base), static_cast<const T*>(scale), shift, out, numel, inner, axis_mode, qmax, zp_signed);
-  } else {
-    quantize_affine_kernel<T, ZP, 1><<<fz_grid(numel, 16), kFzThreads, 0, stream>>>(
-        static_cast<const T*>(base), static_cast<const T*>(scale), shift, out, numel, inner, axis_mode, qmax, zp_signed);
-  }
-  return cudaGetLastError() == cudaSuccess ? OK : ERR_CUDA;
-}
-
-template <typename T>
-static int launch_qa(const void* base, const void* scale, const void* shift, uint8_t* out, int64_t numel, int64_t inner,
-                     int axis_mode, float qmax, int shift_is_int, cudaStream_t stream) {
-  const int zp_signed = shift_is_int == 2 ? 1 : 0;
-  return shift_is_int != 0 ? launch_qa_t<T, true>(base, scale, shift, out, numel, inner, axis_mode, qmax, zp_signed, stream)
-                           : launch_qa_t<T, false>(base, scale, shift, out, numel, inner, axis_mode, qmax, 0, stream);
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // pack: out[i] = OR_p (in[p * plane + i] << bits*p) truncated to a byte, i < plane = R * cols, R = ceil(rows / planes);
 // source bytes beyond rows*cols count as zero (the reference ORs a shorter last slice, packed.py:64-67).
@@ -154,25 +120,6 @@ __global__ void __launch_bounds__(kFzThreads)
     }
     out[i] = static_cast<uint8_t>(acc);
   }
-}
-
-static int launch_pack(const uint8_t* in, uint8_t* out, int64_t rows, int64_t cols, int bits, cudaStream_t stream) {
-  const int planes = 8 / bits;
-  const int64_t packed_rows = (rows + planes - 1) / planes;
-  const int64_t plane = packed_rows * cols, total = rows * cols;
-  if (plane == 0) return OK;
-  const bool vec = (plane % 16 == 0) && (total % 16 == 0) && (reinterpret_cast<uintptr_t>(in) % 16 == 0) &&
-                   (reinterpret_cast<uintptr_t>(out) % 16 == 0);
-  if (vec) {
-    const int grid = fz_grid(plane / 16, 16);
-    if (bits == 4) pack_vec_kernel<4><<<grid, kFzThreads, 0, stream>>>(reinterpret_cast<const uint4*>(in), reinterpret_cast<uint4*>(out), plane / 16, total / 16);
-    else pack_vec_kernel<2><<<grid, kFzThreads, 0, stream>>>(reinterpret_cast<const uint4*>(in), reinterpret_cast<uint4*>(out), plane / 16, total / 16);
-  } else {
-    const int grid = fz_grid(plane, 16);
-    if (bits == 4) pack_scalar_kernel<4><<<grid, kFzThreads, 0, stream>>>(in, out, plane, total);
-    else pack_scalar_kernel<2><<<grid, kFzThreads, 0, stream>>>(in, out, plane, total);
-  }
-  return cudaGetLastError() == cudaSuccess ? OK : ERR_CUDA;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -371,40 +318,6 @@ __global__ void __launch_bounds__(kFzThreads, BITS == 4 ? 4 : 2)
   }
 }
 
-template <typename T, int BITS, bool ZP>
-static int launch_qqm_tl(const void* base, uint8_t* packed, void* scale, void* shift, int64_t rows, int64_t packed_rows,
-                         int group, cudaStream_t stream) {
-  const int lanes = group / 8;
-  int tl = 1;
-  while (tl < lanes) tl <<= 1;
-  const int grid = fz_grid(packed_rows * tl, 8);
-  const T* b = static_cast<const T*>(base);
-  T* s = static_cast<T*>(scale);
-#define QB_QQM(TLV) \
-  quantize_qbits_max_kernel<T, BITS, ZP, TLV><<<grid, kFzThreads, 0, stream>>>(b, packed, s, shift, rows, packed_rows, group)
-  switch (tl) {
-    case 1: QB_QQM(1); break;
-    case 2: QB_QQM(2); break;
-    case 4: QB_QQM(4); break;
-    case 8: QB_QQM(8); break;
-    case 16: QB_QQM(16); break;
-    default: QB_QQM(32); break;
-  }
-#undef QB_QQM
-  return cudaGetLastError() == cudaSuccess ? OK : ERR_CUDA;
-}
-
-template <typename T>
-static int launch_qqm(const void* base, uint8_t* packed, void* scale, void* shift, int64_t rows, int64_t packed_rows,
-                      int group, int bits, bool zp, cudaStream_t stream) {
-  if (bits == 4) {
-    return zp ? launch_qqm_tl<T, 4, true>(base, packed, scale, shift, rows, packed_rows, group, stream)
-              : launch_qqm_tl<T, 4, false>(base, packed, scale, shift, rows, packed_rows, group, stream);
-  }
-  return zp ? launch_qqm_tl<T, 2, true>(base, packed, scale, shift, rows, packed_rows, group, stream)
-            : launch_qqm_tl<T, 2, false>(base, packed, scale, shift, rows, packed_rows, group, stream);
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // absmax (per tensor): out[0] = max |base| as float32.  Non-negative floats order like their bit patterns, so the
 // cross-CTA step is one atomicMax on the int view; `out` is zeroed on the stream by the launcher.
@@ -567,23 +480,6 @@ __global__ void __launch_bounds__(kFzThreads)
   }
 }
 
-template <typename T>
-static int launch_qqa(const void* base, void* out, void* scale, int64_t n, int64_t k, int out_dt, cudaStream_t stream) {
-  const int vec_ok = (k % 8 == 0) && (reinterpret_cast<uintptr_t>(base) % 16 == 0) &&
-                     (reinterpret_cast<uintptr_t>(out) % 8 == 0);
-  const int grid = static_cast<int>(n < static_cast<int64_t>(kNumSMsH100) * 8 ? n : static_cast<int64_t>(kNumSMsH100) * 8);
-  const T* b = static_cast<const T*>(base);
-  uint8_t* o = static_cast<uint8_t*>(out);
-  T* s = static_cast<T*>(scale);
-  switch (out_dt) {
-    case DT_I8: quantize_qbytes_absmax_kernel<T, DT_I8><<<grid, kFzThreads, 0, stream>>>(b, o, s, n, k, 127.f, vec_ok); break;
-    case DT_E4M3: quantize_qbytes_absmax_kernel<T, DT_E4M3><<<grid, kFzThreads, 0, stream>>>(b, o, s, n, k, 448.f, vec_ok); break;
-    case DT_E5M2: quantize_qbytes_absmax_kernel<T, DT_E5M2><<<grid, kFzThreads, 0, stream>>>(b, o, s, n, k, 57344.f, vec_ok); break;
-    default: return ERR_ARG;
-  }
-  return cudaGetLastError() == cudaSuccess ? OK : ERR_CUDA;
-}
-
 }  // namespace qb
 
 using namespace qb;
@@ -592,114 +488,146 @@ extern "C" {
 
 int qb200_quantize_affine(const void* base, const void* scale, const void* shift, uint8_t* out, int64_t outer,
                           int64_t inner, int axis_mode, int bits, int dtype, int shift_is_int, void* stream) {
-  if (bits < 1 || bits > 8) return set_error(ERR_ARG, "quantize_affine: bits must be in 1..8, got %d", bits);
+  if (bits < 1 || bits > 8) return fail(ERR_ARG, "quantize_affine: bits must be in 1..8, got %d", bits);
   if (outer < 0 || inner < 0 || axis_mode < 0 || axis_mode > 2)
-    return set_error(ERR_ARG, "quantize_affine: bad shape / axis_mode (%lld x %lld, mode %d)", (long long)outer,
-                     (long long)inner, axis_mode);
+    return fail(ERR_ARG, "quantize_affine: bad shape / axis_mode (%lld x %lld, mode %d)", (long long)outer,
+                (long long)inner, axis_mode);
   const int64_t numel = outer * inner;
   if (numel == 0) return OK;
-  if (!base || !scale || !shift || !out) return set_error(ERR_ARG, "quantize_affine: null buffer");
+  if (!base || !scale || !shift || !out) return fail(ERR_ARG, "quantize_affine: null buffer");
+  if (!is_float_dtype(dtype)) return fail(ERR_ARG, "quantize_affine: dtype %d not floating point", dtype);
   const float qmax = static_cast<float>((1 << bits) - 1);
+  const int zp_signed = shift_is_int == 2 ? 1 : 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc;
-  switch (dtype) {
-    case DT_F32: rc = launch_qa<float>(base, scale, shift, out, numel, inner, axis_mode, qmax, shift_is_int, st); break;
-    case DT_F16: rc = launch_qa<__half>(base, scale, shift, out, numel, inner, axis_mode, qmax, shift_is_int, st); break;
-    case DT_BF16: rc = launch_qa<__nv_bfloat16>(base, scale, shift, out, numel, inner, axis_mode, qmax, shift_is_int, st); break;
-    default: return set_error(ERR_ARG, "quantize_affine: dtype %d not floating point", dtype);
-  }
-  return rc == OK ? OK : set_error(rc, "quantize_affine: launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+  const bool vec = inner % 8 == 0 && aligned16(base) && reinterpret_cast<uintptr_t>(out) % 8 == 0;
+  return dispatch_float(dtype, [&](auto dt) {
+    return dispatch_zp(shift_is_int, [&](auto ZP) {
+      using T = typename decltype(dt)::T;
+      const T* b = static_cast<const T*>(base);
+      const T* s = static_cast<const T*>(scale);
+      if (vec)
+        quantize_affine_kernel<T, ZP, 8><<<capped_grid(numel / 8, kFzThreads, 16), kFzThreads, 0, st>>>(
+            b, s, shift, out, numel, inner, axis_mode, qmax, ZP ? zp_signed : 0);
+      else
+        quantize_affine_kernel<T, ZP, 1><<<capped_grid(numel, kFzThreads, 16), kFzThreads, 0, st>>>(
+            b, s, shift, out, numel, inner, axis_mode, qmax, ZP ? zp_signed : 0);
+      return check_cuda(cudaGetLastError(), "quantize_affine launch");
+    });
+  });
 }
 
 int qb200_pack(const uint8_t* in, uint8_t* out, int64_t rows, int64_t cols, int bits, void* stream) {
-  if (bits != 2 && bits != 4) return set_error(ERR_ARG, "pack: bits must be 2 or 4, got %d", bits);
-  if (rows < 0 || cols < 0) return set_error(ERR_ARG, "pack: negative shape");
-  if (rows * cols > 0 && (!in || !out)) return set_error(ERR_ARG, "pack: null buffer");
-  int rc = launch_pack(in, out, rows, cols, bits, static_cast<cudaStream_t>(stream));
-  return rc == OK ? OK : set_error(rc, "pack: launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+  if (bits != 2 && bits != 4) return fail(ERR_ARG, "pack: bits must be 2 or 4, got %d", bits);
+  if (rows < 0 || cols < 0) return fail(ERR_ARG, "pack: negative shape");
+  if (rows * cols > 0 && (!in || !out)) return fail(ERR_ARG, "pack: null buffer");
+  const int planes = 8 / bits;
+  const int64_t packed_rows = (rows + planes - 1) / planes;
+  const int64_t plane = packed_rows * cols, total = rows * cols;
+  if (plane == 0) return OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool vec = plane % 16 == 0 && total % 16 == 0 && aligned16(in) && aligned16(out);
+  return dispatch_bits(bits, [&](auto BITS) {
+    if (vec)
+      pack_vec_kernel<BITS><<<capped_grid(plane / 16, kFzThreads, 16), kFzThreads, 0, st>>>(
+          reinterpret_cast<const uint4*>(in), reinterpret_cast<uint4*>(out), plane / 16, total / 16);
+    else
+      pack_scalar_kernel<BITS><<<capped_grid(plane, kFzThreads, 16), kFzThreads, 0, st>>>(in, out, plane, total);
+    return check_cuda(cudaGetLastError(), "pack launch");
+  });
 }
 
 int qb200_quantize_qbits_max(const void* base, uint8_t* packed, void* scale, void* shift, int64_t n, int64_t k,
                              int group, int bits, int dtype, int zeropoint, void* stream) {
-  if (bits != 2 && bits != 4) return set_error(ERR_ARG, "quantize_qbits_max: bits must be 2 or 4, got %d", bits);
-  if (n <= 0 || k <= 0 || group <= 0) return set_error(ERR_ARG, "quantize_qbits_max: bad shape");
-  if (k % group != 0) return set_error(ERR_ARG, "quantize_qbits_max: group %d does not divide K=%lld", group, (long long)k);
+  if (bits != 2 && bits != 4) return fail(ERR_ARG, "quantize_qbits_max: bits must be 2 or 4, got %d", bits);
+  if (n <= 0 || k <= 0 || group <= 0) return fail(ERR_ARG, "quantize_qbits_max: bad shape");
+  if (k % group != 0) return fail(ERR_ARG, "quantize_qbits_max: group %d does not divide K=%lld", group, (long long)k);
   if (group % 8 != 0 || group > 256)
-    return set_error(ERR_UNSUPPORTED, "quantize_qbits_max: group %d (needs a multiple of 8, <= 256)", group);
-  if (!base || !packed || !scale || !shift) return set_error(ERR_ARG, "quantize_qbits_max: null buffer");
-  if (reinterpret_cast<uintptr_t>(base) % 16 != 0 || reinterpret_cast<uintptr_t>(packed) % 8 != 0)
-    return set_error(ERR_UNSUPPORTED, "quantize_qbits_max: base must be 16-byte and packed 8-byte aligned");
+    return fail(ERR_UNSUPPORTED, "quantize_qbits_max: group %d (needs a multiple of 8, <= 256)", group);
+  if (!base || !packed || !scale || !shift) return fail(ERR_ARG, "quantize_qbits_max: null buffer");
+  if (!aligned16(base) || reinterpret_cast<uintptr_t>(packed) % 8 != 0)
+    return fail(ERR_UNSUPPORTED, "quantize_qbits_max: base must be 16-byte and packed 8-byte aligned");
+  if (!is_float_dtype(dtype)) return fail(ERR_ARG, "quantize_qbits_max: dtype %d not floating point", dtype);
   const int64_t rows = n * k / group;
   const int planes = 8 / bits;
   const int64_t packed_rows = (rows + planes - 1) / planes;
+  const int grid = capped_grid(packed_rows * team_lanes(group), kFzThreads, 8);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc;
-  switch (dtype) {
-    case DT_F32: rc = launch_qqm<float>(base, packed, scale, shift, rows, packed_rows, group, bits, zeropoint != 0, st); break;
-    case DT_F16: rc = launch_qqm<__half>(base, packed, scale, shift, rows, packed_rows, group, bits, zeropoint != 0, st); break;
-    case DT_BF16: rc = launch_qqm<__nv_bfloat16>(base, packed, scale, shift, rows, packed_rows, group, bits, zeropoint != 0, st); break;
-    default: return set_error(ERR_ARG, "quantize_qbits_max: dtype %d not floating point", dtype);
-  }
-  return rc == OK ? OK : set_error(rc, "quantize_qbits_max: launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+  return dispatch_float(dtype, [&](auto dt) {
+    return dispatch_bits(bits, [&](auto BITS) {
+      return dispatch_zp(zeropoint, [&](auto ZP) {
+        return dispatch_team_lanes(group, [&](auto TL) {
+          using T = typename decltype(dt)::T;
+          quantize_qbits_max_kernel<T, BITS, ZP, TL><<<grid, kFzThreads, 0, st>>>(
+              static_cast<const T*>(base), packed, static_cast<T*>(scale), shift, rows, packed_rows, group);
+          return check_cuda(cudaGetLastError(), "quantize_qbits_max launch");
+        });
+      });
+    });
+  });
 }
 
 int qb200_absmax(const void* base, void* out, void* scratch, int64_t numel, int dtype, void* stream) {
-  if (numel < 0 || !out || !scratch || (numel > 0 && !base)) return set_error(ERR_ARG, "absmax: bad buffer");
-  if (reinterpret_cast<uintptr_t>(scratch) % 4 != 0) return set_error(ERR_ARG, "absmax: scratch must be 4-byte aligned");
+  if (numel < 0 || !out || !scratch || (numel > 0 && !base)) return fail(ERR_ARG, "absmax: bad buffer");
+  if (reinterpret_cast<uintptr_t>(scratch) % 4 != 0) return fail(ERR_ARG, "absmax: scratch must be 4-byte aligned");
+  if (!is_float_dtype(dtype)) return fail(ERR_ARG, "absmax: dtype %d not floating point", dtype);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (cudaMemsetAsync(scratch, 0, 8, st) != cudaSuccess) return set_error(ERR_CUDA, "absmax: memset failed");
-  const int vec_ok = reinterpret_cast<uintptr_t>(base) % 16 == 0;
-  const int grid = numel == 0 ? 1 : fz_grid((numel + 15) / 16, 8);
-  int* sc = static_cast<int*>(scratch);
-  switch (dtype) {
-    case DT_F32: absmax_kernel<float><<<grid, kFzThreads, 0, st>>>(static_cast<const float*>(base), static_cast<float*>(out), sc, numel, vec_ok); break;
-    case DT_F16: absmax_kernel<__half><<<grid, kFzThreads, 0, st>>>(static_cast<const __half*>(base), static_cast<__half*>(out), sc, numel, vec_ok); break;
-    case DT_BF16: absmax_kernel<__nv_bfloat16><<<grid, kFzThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(base), static_cast<__nv_bfloat16*>(out), sc, numel, vec_ok); break;
-    default: return set_error(ERR_ARG, "absmax: dtype %d not floating point", dtype);
-  }
-  return cudaGetLastError() == cudaSuccess ? OK : set_error(ERR_CUDA, "absmax: launch failed");
+  int rc = check_cuda(cudaMemsetAsync(scratch, 0, 8, st), "absmax: scratch memset");
+  if (rc != OK) return rc;
+  const int vec_ok = aligned16(base);
+  const int grid = capped_grid((numel + 15) / 16, kFzThreads, 8);
+  return dispatch_float(dtype, [&](auto dt) {
+    using T = typename decltype(dt)::T;
+    absmax_kernel<T><<<grid, kFzThreads, 0, st>>>(static_cast<const T*>(base), static_cast<T*>(out),
+                                                  static_cast<int*>(scratch), numel, vec_ok);
+    return check_cuda(cudaGetLastError(), "absmax launch");
+  });
 }
 
 int qb200_absmax_update(const void* base, void* scale, void* scratch, int64_t numel, int dtype, double qmax,
                         double momentum, void* stream) {
-  if (numel < 1) return set_error(ERR_ARG, "absmax_update: the tensor is empty (numel %lld)", (long long)numel);
-  if (!base || !scale || !scratch) return set_error(ERR_ARG, "absmax_update: null buffer");
-  if (reinterpret_cast<uintptr_t>(scratch) % 4 != 0)
-    return set_error(ERR_ARG, "absmax_update: scratch must be 4-byte aligned");
-  if (!(qmax > 0.0)) return set_error(ERR_ARG, "absmax_update: qmax must be positive");
+  if (numel < 1) return fail(ERR_ARG, "absmax_update: the tensor is empty (numel %lld)", (long long)numel);
+  if (!base || !scale || !scratch) return fail(ERR_ARG, "absmax_update: null buffer");
+  if (reinterpret_cast<uintptr_t>(scratch) % 4 != 0) return fail(ERR_ARG, "absmax_update: scratch must be 4-byte aligned");
+  if (!(qmax > 0.0)) return fail(ERR_ARG, "absmax_update: qmax must be positive");
+  if (!is_float_dtype(dtype)) return fail(ERR_ARG, "absmax_update: dtype %d not floating point", dtype);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int vec_ok = reinterpret_cast<uintptr_t>(base) % 16 == 0;
-  const int grid = fz_grid((numel + 15) / 16, 8);
-  int* sc = static_cast<int*>(scratch);
+  int rc = check_cuda(cudaMemsetAsync(scratch, 0, 8, st), "absmax_update: scratch memset");
+  if (rc != OK) return rc;
+  const int vec_ok = aligned16(base);
+  const int grid = capped_grid((numel + 15) / 16, kFzThreads, 8);
   // the python scalars become float operands of ATen's float opmath: momentum, and 1 - momentum evaluated in double
   const float q = static_cast<float>(qmax), m = static_cast<float>(momentum), om = static_cast<float>(1.0 - momentum);
-  if (dtype != DT_F32 && dtype != DT_F16 && dtype != DT_BF16)
-    return set_error(ERR_ARG, "absmax_update: dtype %d not floating point", dtype);
-  if (cudaMemsetAsync(scratch, 0, 8, st) != cudaSuccess) return set_error(ERR_CUDA, "absmax_update: memset failed");
-  switch (dtype) {
-    case DT_F32: absmax_update_kernel<float><<<grid, kFzThreads, 0, st>>>(static_cast<const float*>(base), static_cast<float*>(scale), sc, numel, vec_ok, q, m, om); break;
-    case DT_F16: absmax_update_kernel<__half><<<grid, kFzThreads, 0, st>>>(static_cast<const __half*>(base), static_cast<__half*>(scale), sc, numel, vec_ok, q, m, om); break;
-    default: absmax_update_kernel<__nv_bfloat16><<<grid, kFzThreads, 0, st>>>(static_cast<const __nv_bfloat16*>(base), static_cast<__nv_bfloat16*>(scale), sc, numel, vec_ok, q, m, om); break;
-  }
-  return cudaGetLastError() == cudaSuccess ? OK : set_error(ERR_CUDA, "absmax_update: launch failed");
+  return dispatch_float(dtype, [&](auto dt) {
+    using T = typename decltype(dt)::T;
+    absmax_update_kernel<T><<<grid, kFzThreads, 0, st>>>(static_cast<const T*>(base), static_cast<T*>(scale),
+                                                         static_cast<int*>(scratch), numel, vec_ok, q, m, om);
+    return check_cuda(cudaGetLastError(), "absmax_update launch");
+  });
 }
 
 int qb200_quantize_qbytes_absmax(const void* base, void* out, void* scale, int64_t n, int64_t k, int dtype,
                                  int out_dtype, void* stream) {
-  if (n < 0 || k < 0) return set_error(ERR_ARG, "quantize_qbytes_absmax: negative shape");
+  if (n < 0 || k < 0) return fail(ERR_ARG, "quantize_qbytes_absmax: negative shape");
   if (n == 0 || k == 0) return OK;
-  if (!base || !out || !scale) return set_error(ERR_ARG, "quantize_qbytes_absmax: null buffer");
-  if (out_dtype != DT_I8 && out_dtype != DT_E4M3 && out_dtype != DT_E5M2)
-    return set_error(ERR_ARG, "quantize_qbytes_absmax: unsupported target dtype %d", out_dtype);
+  if (!base || !out || !scale) return fail(ERR_ARG, "quantize_qbytes_absmax: null buffer");
+  if (!is_code_dtype(out_dtype)) return fail(ERR_ARG, "quantize_qbytes_absmax: unsupported target dtype %d", out_dtype);
+  if (!is_float_dtype(dtype)) return fail(ERR_ARG, "quantize_qbytes_absmax: dtype %d not floating point", dtype);
+  const int vec_ok = k % 8 == 0 && aligned16(base) && reinterpret_cast<uintptr_t>(out) % 8 == 0;
+  const float qmax = out_dtype == DT_I8 ? 127.f : (out_dtype == DT_E4M3 ? 448.f : 57344.f);
+  const int grid = capped_grid(n, 1, 8);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc;
-  switch (dtype) {
-    case DT_F32: rc = launch_qqa<float>(base, out, scale, n, k, out_dtype, st); break;
-    case DT_F16: rc = launch_qqa<__half>(base, out, scale, n, k, out_dtype, st); break;
-    case DT_BF16: rc = launch_qqa<__nv_bfloat16>(base, out, scale, n, k, out_dtype, st); break;
-    default: return set_error(ERR_ARG, "quantize_qbytes_absmax: dtype %d not floating point", dtype);
-  }
-  return rc == OK ? OK : set_error(rc, "quantize_qbytes_absmax: launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+  return dispatch_float(dtype, [&](auto dt) {
+    return dispatch_code8(out_dtype, [&](auto OUT) {
+      using T = typename decltype(dt)::T;
+      if constexpr (decltype(OUT)::value == DT_E4M3FNUZ) {  // no kernel: int8, e4m3fn and e5m2 targets only
+        return fail(ERR_ARG, "quantize_qbytes_absmax: unsupported target dtype %d", out_dtype);
+      } else {
+        quantize_qbytes_absmax_kernel<T, OUT><<<grid, kFzThreads, 0, st>>>(
+            static_cast<const T*>(base), static_cast<uint8_t*>(out), static_cast<T*>(scale), n, k, qmax, vec_ok);
+        return check_cuda(cudaGetLastError(), "quantize_qbytes_absmax launch");
+      }
+    });
+  });
 }
 
 }  // extern "C"

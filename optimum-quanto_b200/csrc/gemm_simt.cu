@@ -3,7 +3,7 @@
 // order literally (optimum/quanto/library/qbytes_mm.py:25-50):
 //   int8 x int8 : acc = int32 sum ; out = rnd_T(fp32(acc) * fp32(scale[n]))
 //   otherwise   : A' = rnd_T(A) ; Ws = rnd_T(scale[n] * W) ; out = rnd_T(sum_k A'*Ws)  (fp32 accumulate)
-#include "common.cuh"
+#include "host_common.cuh"
 
 namespace qb {
 
@@ -86,30 +86,20 @@ __global__ void __launch_bounds__(256)
     }
 }
 
-template <typename T>
-static int launch_simt_t(const void* A, const void* W, const void* scales, const void* bias, void* out, int M, int N,
-                         int K, int a_dt, int w_dt, cudaStream_t stream) {
-  dim3 grid((N + ST - 1) / ST, (M + ST - 1) / ST);
-  const bool int_path = (a_dt == DT_I8 && w_dt == DT_I8);
-  if (int_path)
-    qbytes_mm_simt_kernel<T, true><<<grid, 256, 0, stream>>>(A, W, static_cast<const T*>(scales),
-                                                             static_cast<const T*>(bias), static_cast<T*>(out), M, N,
-                                                             K, a_dt, w_dt);
-  else
-    qbytes_mm_simt_kernel<T, false><<<grid, 256, 0, stream>>>(A, W, static_cast<const T*>(scales),
-                                                              static_cast<const T*>(bias), static_cast<T*>(out), M, N,
-                                                              K, a_dt, w_dt);
-  return cudaGetLastError() == cudaSuccess ? OK : ERR_CUDA;
-}
-
 int launch_qbytes_mm_simt(const void* A, const void* W, const void* scales, const void* bias, void* out, int M, int N,
                           int K, int a_dt, int w_dt, int out_dt, cudaStream_t stream) {
-  switch (out_dt) {
-    case DT_F32: return launch_simt_t<float>(A, W, scales, bias, out, M, N, K, a_dt, w_dt, stream);
-    case DT_F16: return launch_simt_t<__half>(A, W, scales, bias, out, M, N, K, a_dt, w_dt, stream);
-    case DT_BF16: return launch_simt_t<__nv_bfloat16>(A, W, scales, bias, out, M, N, K, a_dt, w_dt, stream);
-    default: return ERR_ARG;
-  }
+  dim3 grid((N + ST - 1) / ST, (M + ST - 1) / ST);
+  const bool int_path = a_dt == DT_I8 && w_dt == DT_I8;
+  return dispatch_float(out_dt, [&](auto dt) {
+    using T = typename decltype(dt)::T;
+    auto launch = [&](auto INT_PATH) {
+      qbytes_mm_simt_kernel<T, INT_PATH><<<grid, 256, 0, stream>>>(A, W, static_cast<const T*>(scales),
+                                                                   static_cast<const T*>(bias), static_cast<T*>(out), M,
+                                                                   N, K, a_dt, w_dt);
+      return check_cuda(cudaGetLastError(), "qbytes_mm CUDA-core launch");
+    };
+    return int_path ? launch(std::true_type{}) : launch(std::false_type{});
+  });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -185,35 +175,23 @@ __global__ void __launch_bounds__(256)
     }
 }
 
-template <typename T>
-static int launch_qbits_simt_t(const void* x, const uint8_t* packed, const void* scale, const void* shift,
-                               const void* bias, void* out, int M, int N, int K, int group, int bits, int shift_is_int,
-                               int64_t ld, int64_t col0, cudaStream_t stream) {
+int launch_qbits_mm_simt(const void* x, const uint8_t* packed, const void* scale, const void* shift, const void* bias,
+                         void* out, int M, int N, int K, int group, int bits, int dt, int shift_is_int, int64_t ld,
+                         int64_t col0, cudaStream_t stream) {
   dim3 grid((N + ST - 1) / ST, (M + ST - 1) / ST);
   const int64_t rows = static_cast<int64_t>(N) * (K / group);
   const int planes = 8 / bits;
   const int64_t packed_rows = (rows + planes - 1) / planes;
-  if (bits == 4)
-    qbits_mm_simt_kernel<T, 4><<<grid, 256, 0, stream>>>(static_cast<const T*>(x), packed, static_cast<const T*>(scale),
-                                                         shift, static_cast<const T*>(bias), static_cast<T*>(out), M, N,
-                                                         K, group, packed_rows, shift_is_int, ld, col0);
-  else
-    qbits_mm_simt_kernel<T, 2><<<grid, 256, 0, stream>>>(static_cast<const T*>(x), packed, static_cast<const T*>(scale),
-                                                         shift, static_cast<const T*>(bias), static_cast<T*>(out), M, N,
-                                                         K, group, packed_rows, shift_is_int, ld, col0);
-  return cudaGetLastError() == cudaSuccess ? OK : ERR_CUDA;
-}
-
-int launch_qbits_mm_simt(const void* x, const uint8_t* packed, const void* scale, const void* shift, const void* bias,
-                         void* out, int M, int N, int K, int group, int bits, int dt, int shift_is_int, int64_t ld,
-                         int64_t col0, cudaStream_t stream) {
-  if ((bits != 2 && bits != 4) || group <= 0 || K % group != 0) return ERR_ARG;
-  switch (dt) {
-    case DT_F32: return launch_qbits_simt_t<float>(x, packed, scale, shift, bias, out, M, N, K, group, bits, shift_is_int, ld, col0, stream);
-    case DT_F16: return launch_qbits_simt_t<__half>(x, packed, scale, shift, bias, out, M, N, K, group, bits, shift_is_int, ld, col0, stream);
-    case DT_BF16: return launch_qbits_simt_t<__nv_bfloat16>(x, packed, scale, shift, bias, out, M, N, K, group, bits, shift_is_int, ld, col0, stream);
-    default: return ERR_ARG;
-  }
+  return dispatch_float(dt, [&](auto t) {
+    return dispatch_bits(bits, [&](auto BITS) {
+      using T = typename decltype(t)::T;
+      qbits_mm_simt_kernel<T, BITS><<<grid, 256, 0, stream>>>(static_cast<const T*>(x), packed,
+                                                              static_cast<const T*>(scale), shift,
+                                                              static_cast<const T*>(bias), static_cast<T*>(out), M, N,
+                                                              K, group, packed_rows, shift_is_int, ld, col0);
+      return check_cuda(cudaGetLastError(), "qbits_mm CUDA-core launch");
+    });
+  });
 }
 
 }  // namespace qb

@@ -14,6 +14,8 @@ namespace qb {
 
 // ---- status (defined in api_core.cu; the message is thread-local, read back through qb200_last_error) ----------
 int fail(int code, const char* fmt, ...);
+// OK, or ERR_CUDA with the message "<what>: <the runtime's reason>".  Launchers pass cudaGetLastError() straight in:
+// that call clears a non-sticky error, so a later call could no longer report it.
 int check_cuda(cudaError_t e, const char* what);
 void set_kernel_family(int family);
 
@@ -23,7 +25,7 @@ void set_kernel_family(int family);
 constexpr int kMaxDevices = 64;
 int current_device();       // cudaGetDevice, -1 on error
 int current_sm_count();     // multiprocessors of the current device
-int check_arch();           // OK when the current device is sm_90 (Hopper), else ERR_ARCH (message set)
+int check_arch(const char* what);  // OK when the current device is sm_90 (Hopper), else ERR_ARCH / ERR_CUDA
 
 // Opt the kernel into `bytes` of dynamic shared memory on the current device (once per kernel and device).  The kernel
 // is a template ARGUMENT: one static per kernel function (kernels of different configurations share a pointer TYPE).
@@ -87,6 +89,24 @@ int make_tmap_3d_bytes(CUtensorMap* map, const void* base, int64_t batch, int64_
 // TMA operands, vector loads and bulk copies need 16-byte aligned addresses
 inline bool aligned16(const void* ptr) { return reinterpret_cast<uintptr_t>(ptr) % 16 == 0; }
 
+// Grid of a grid-stride kernel: one CTA per `per_cta` work items, at least 1 and at most `ctas_per_sm` CTAs for each SM
+// of a 132-SM H100 SXM.
+inline int capped_grid(int64_t items, int64_t per_cta, int ctas_per_sm) {
+  const int64_t blocks = (items + per_cta - 1) / per_cta;
+  const int64_t cap = static_cast<int64_t>(kNumSMsH100) * ctas_per_sm;
+  return static_cast<int>(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
+}
+
+inline bool is_float_dtype(int dt) { return dt == DT_F32 || dt == DT_F16 || dt == DT_BF16; }
+inline bool is_code_dtype(int dt) { return dt == DT_I8 || dt == DT_E4M3 || dt == DT_E5M2 || dt == DT_E4M3FNUZ; }
+
+// Lanes of the team that owns one grouped row of `group` elements (8 per lane): group / 8 rounded up to a power of two
+inline int team_lanes(int group) {
+  int tl = 1;
+  while (tl < group / 8) tl <<= 1;
+  return tl;
+}
+
 // ---- run-time codes -> template arguments.  Each dispatch_* helper calls the generic lambda `f` with a tag type for the
 // code it is given, so that `f` names the kernel configuration once and instantiates it for exactly the codes listed
 // here.  The entry points validate their arguments first: a code outside a helper's set is a dispatch bug, reported as
@@ -138,6 +158,57 @@ int dispatch_mwg(int tile_m, F&& f) {
   if (tile_m == 64) return f(std::integral_constant<int, 1>{});
   if (tile_m == 128) return f(std::integral_constant<int, 2>{});
   return fail(ERR_ARG, "dispatch: tile height %d is neither 64 nor 128", tile_m);
+}
+
+// float element dtype: the element type T
+template <typename T_>
+struct Float {
+  using T = T_;
+};
+
+// DT_F32 / DT_F16 / DT_BF16 -> Float<float> / Float<__half> / Float<__nv_bfloat16>
+template <class F>
+int dispatch_float(int dtype, F&& f) {
+  switch (dtype) {
+    case DT_F32: return f(Float<float>{});
+    case DT_F16: return f(Float<__half>{});
+    case DT_BF16: return f(Float<__nv_bfloat16>{});
+    default: return fail(ERR_ARG, "dispatch: dtype %d is not a float type", dtype);
+  }
+}
+
+// 8-bit code dtype -> std::integral_constant<int, DT_*>
+template <class F>
+int dispatch_code8(int dtype, F&& f) {
+  switch (dtype) {
+    case DT_I8: return f(std::integral_constant<int, DT_I8>{});
+    case DT_E4M3: return f(std::integral_constant<int, DT_E4M3>{});
+    case DT_E5M2: return f(std::integral_constant<int, DT_E5M2>{});
+    case DT_E4M3FNUZ: return f(std::integral_constant<int, DT_E4M3FNUZ>{});
+    default: return fail(ERR_ARG, "dispatch: dtype %d is not an 8-bit code type", dtype);
+  }
+}
+
+// bits per packed weight 2 / 4 -> std::integral_constant BITS
+template <class F>
+int dispatch_bits(int bits, F&& f) {
+  if (bits == 4) return f(std::integral_constant<int, 4>{});
+  if (bits == 2) return f(std::integral_constant<int, 2>{});
+  return fail(ERR_ARG, "dispatch: bits %d is neither 2 nor 4", bits);
+}
+
+// group (a multiple of 8, at most 256) -> std::integral_constant TL = team_lanes(group) in 1 ... 32
+template <class F>
+int dispatch_team_lanes(int group, F&& f) {
+  switch (team_lanes(group)) {
+    case 1: return f(std::integral_constant<int, 1>{});
+    case 2: return f(std::integral_constant<int, 2>{});
+    case 4: return f(std::integral_constant<int, 4>{});
+    case 8: return f(std::integral_constant<int, 8>{});
+    case 16: return f(std::integral_constant<int, 16>{});
+    case 32: return f(std::integral_constant<int, 32>{});
+    default: return fail(ERR_ARG, "dispatch: group %d needs more than 32 lanes", group);
+  }
 }
 
 // ---- test hooks (include/quanto_b200.h: qb200_test_override).  Every value selects a kernel that computes the same

@@ -23,12 +23,11 @@
 #include <type_traits>
 
 #include "../../include/quanto_b200.h"
-#include "common.cuh"
+
+#include "host_common.cuh"
 #include "quantize_math.cuh"
 
 namespace qb {
-
-int set_error(int code, const char* fmt, ...);
 
 constexpr int kHqqThreads = 256;
 constexpr int kHqqWarps = kHqqThreads / 32;
@@ -282,17 +281,8 @@ __global__ void __launch_bounds__(kHqqThreads)
 }
 
 // ----------------------------------------------------------------------------------------------------- host side
-static int hqq_team_lanes(int group) {
-  int tl = 1;
-  while (tl < group / 8) tl <<= 1;
-  return tl;
-}
-
 static int hqq_search_grid(int64_t rows, int group) {
-  const int64_t teams_per_cta = kHqqThreads / hqq_team_lanes(group);
-  int64_t blocks = (rows + teams_per_cta - 1) / teams_per_cta;
-  const int64_t cap = static_cast<int64_t>(kNumSMsH100) * kHqqCtasPerSm;
-  return static_cast<int>(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
+  return capped_grid(rows, kHqqThreads / team_lanes(group), kHqqCtasPerSm);
 }
 
 static size_t align256(size_t b) { return (b + 255) & ~static_cast<size_t>(255); }
@@ -309,76 +299,34 @@ static HqqLayout hqq_layout(int64_t rows, int group, int iters, int elem_bytes) 
   return l;
 }
 
+// dynamic shared memory of the pow table: none for lp_norm == 1 (LP1), which needs no power
+template <typename T, bool LP1>
+static int table_smem() {
+  return LP1 ? 0 : kHqqTable * static_cast<int>(sizeof(T));
+}
+
+// opts `kern` into `smem` bytes of dynamic shared memory when it uses any
+template <class Kernel>
+static int opt_into_table(Kernel kern, int smem, const char* what) {
+  if (smem == 0) return OK;
+  return check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem), what);
+}
+
 // the pow exponent torch uses: python's lp_norm - 1 converted to the tensor dtype (through float, as c10 does)
 template <typename T>
 static double hqq_pow_exponent(double lp_norm) {
   return static_cast<double>(static_cast<float>(T(static_cast<float>(lp_norm - 1.0))));
 }
 
-template <typename T, int BITS, bool LP1, int TL>
-static void launch_search_tl(const void* base, void* scale, void* cands, double* partials, HqqHeader* header,
-                             float* errors, int64_t rows, int group, int iters, double pow_exp, double numel,
-                             const HqqParams& P, cudaStream_t st) {
-  auto kern = hqq_search_kernel<T, BITS, TL, LP1>;
-  const int smem = LP1 ? 0 : kHqqTable * static_cast<int>(sizeof(T));
-  if (smem > 0) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  kern<<<hqq_search_grid(rows, group), kHqqThreads, smem, st>>>(
-      static_cast<const T*>(base), static_cast<T*>(scale), static_cast<T*>(cands), partials, header, errors, rows,
-      group, iters, pow_exp, numel, P);
-}
-
-template <typename T, int BITS, bool ZP, int TL>
-static void launch_pack_tl(const void* base, uint8_t* packed, const void* scale, void* shift, const void* cands,
-                           const HqqHeader* header, int64_t rows, int group, cudaStream_t st) {
-  const int64_t packed_rows = (rows + (8 / BITS) - 1) / (8 / BITS);
-  const int64_t teams_per_cta = kHqqThreads / TL;
-  int64_t blocks = (packed_rows + teams_per_cta - 1) / teams_per_cta;
-  const int64_t cap = static_cast<int64_t>(kNumSMsH100) * 8;
-  blocks = blocks > cap ? cap : blocks;
-  hqq_pack_kernel<T, BITS, ZP, TL><<<static_cast<int>(blocks), kHqqThreads, 0, st>>>(
-      static_cast<const T*>(base), packed, static_cast<const T*>(scale), shift, static_cast<const T*>(cands), header,
-      rows, packed_rows, group);
-}
-
-template <typename T, int BITS, int TL>
-static void launch_hqq_tl(const void* base, uint8_t* packed, void* scale, void* shift, float* errors, char* ws,
-                          const HqqLayout& L, int64_t rows, int group, bool zp, bool lp1, int iters, double pow_exp,
-                          double numel, const HqqParams& P, cudaStream_t st) {
-  HqqHeader* header = reinterpret_cast<HqqHeader*>(ws);
-  double* partials = reinterpret_cast<double*>(ws + L.partials);
-  void* cands = ws + L.cands;
-  if (lp1) launch_search_tl<T, BITS, true, TL>(base, scale, cands, partials, header, errors, rows, group, iters, pow_exp, numel, P, st);
-  else launch_search_tl<T, BITS, false, TL>(base, scale, cands, partials, header, errors, rows, group, iters, pow_exp, numel, P, st);
-  if (zp) launch_pack_tl<T, BITS, true, TL>(base, packed, scale, shift, cands, header, rows, group, st);
-  else launch_pack_tl<T, BITS, false, TL>(base, packed, scale, shift, cands, header, rows, group, st);
-}
-
-template <typename T, int BITS>
-static void launch_hqq_bits(int tl, const void* base, uint8_t* packed, void* scale, void* shift, float* errors,
-                            char* ws, const HqqLayout& L, int64_t rows, int group, bool zp, bool lp1, int iters,
-                            double pow_exp, double numel, const HqqParams& P, cudaStream_t st) {
-#define QB_HQQ(TLV) \
-  launch_hqq_tl<T, BITS, TLV>(base, packed, scale, shift, errors, ws, L, rows, group, zp, lp1, iters, pow_exp, numel, P, st)
-  switch (tl) {
-    case 1: QB_HQQ(1); break;
-    case 2: QB_HQQ(2); break;
-    case 4: QB_HQQ(4); break;
-    case 8: QB_HQQ(8); break;
-    case 16: QB_HQQ(16); break;
-    default: QB_HQQ(32); break;
-  }
-#undef QB_HQQ
-}
-
 // ERR_UNSUPPORTED (the caller composes ATen ops) for what the kernel does not reproduce bit for bit
 static int hqq_check_config(const char* what, int dtype, double lp_norm) {
   if (dtype == DT_F32)
-    return set_error(ERR_UNSUPPORTED, "%s: float32 weights (the reference's float32 pow is not correctly rounded)", what);
-  if (dtype != DT_F16 && dtype != DT_BF16) return set_error(ERR_ARG, "%s: dtype %d not floating point", what, dtype);
-  if (!(lp_norm > 0.0)) return set_error(ERR_UNSUPPORTED, "%s: lp_norm must be > 0, got %g", what, lp_norm);
+    return fail(ERR_UNSUPPORTED, "%s: float32 weights (the reference's float32 pow is not correctly rounded)", what);
+  if (dtype != DT_F16 && dtype != DT_BF16) return fail(ERR_ARG, "%s: dtype %d not floating point", what, dtype);
+  if (!(lp_norm > 0.0)) return fail(ERR_UNSUPPORTED, "%s: lp_norm must be > 0, got %g", what, lp_norm);
   const double e = dtype == DT_BF16 ? hqq_pow_exponent<__nv_bfloat16>(lp_norm) : hqq_pow_exponent<__half>(lp_norm);
   if (e == 3.0)  // torch computes x * x * x there, which is not the rounded power
-    return set_error(ERR_UNSUPPORTED, "%s: lp_norm %g (torch.pow special-cases the cube)", what, lp_norm);
+    return fail(ERR_UNSUPPORTED, "%s: lp_norm %g (torch.pow special-cases the cube)", what, lp_norm);
   return OK;
 }
 
@@ -397,79 +345,86 @@ int qb200_quantize_qbits_hqq(const void* base, uint8_t* packed, void* scale, voi
                              void* workspace, int64_t n, int64_t k, int group, int bits, int dtype, int zeropoint,
                              double lp_norm, double beta, double kappa, int iters, void* stream) {
   const char* what = "quantize_qbits_hqq";
-  if (bits != 2 && bits != 4) return set_error(ERR_ARG, "%s: bits must be 2 or 4, got %d", what, bits);
-  if (n <= 0 || k <= 0 || group <= 0) return set_error(ERR_ARG, "%s: bad shape", what);
-  if (k % group != 0) return set_error(ERR_ARG, "%s: group %d does not divide K=%lld", what, group, (long long)k);
-  if (iters < 0) return set_error(ERR_ARG, "%s: iters must be >= 0, got %d", what, iters);
-  const int rc = hqq_check_config(what, dtype, lp_norm);
+  if (bits != 2 && bits != 4) return fail(ERR_ARG, "%s: bits must be 2 or 4, got %d", what, bits);
+  if (n <= 0 || k <= 0 || group <= 0) return fail(ERR_ARG, "%s: bad shape", what);
+  if (k % group != 0) return fail(ERR_ARG, "%s: group %d does not divide K=%lld", what, group, (long long)k);
+  if (iters < 0) return fail(ERR_ARG, "%s: iters must be >= 0, got %d", what, iters);
+  int rc = hqq_check_config(what, dtype, lp_norm);
   if (rc != OK) return rc;
   if (group % 8 != 0 || group > 256)
-    return set_error(ERR_UNSUPPORTED, "%s: group %d (needs a multiple of 8, <= 256)", what, group);
-  if (iters > kHqqMaxIters) return set_error(ERR_UNSUPPORTED, "%s: iters %d > %d", what, iters, kHqqMaxIters);
-  if (!base || !packed || !scale || !shift || !errors || !workspace) return set_error(ERR_ARG, "%s: null buffer", what);
+    return fail(ERR_UNSUPPORTED, "%s: group %d (needs a multiple of 8, <= 256)", what, group);
+  if (iters > kHqqMaxIters) return fail(ERR_UNSUPPORTED, "%s: iters %d > %d", what, iters, kHqqMaxIters);
+  if (!base || !packed || !scale || !shift || !errors || !workspace) return fail(ERR_ARG, "%s: null buffer", what);
   if (reinterpret_cast<uintptr_t>(base) % 16 != 0 || reinterpret_cast<uintptr_t>(packed) % 8 != 0 ||
       reinterpret_cast<uintptr_t>(workspace) % 256 != 0)
-    return set_error(ERR_UNSUPPORTED, "%s: base must be 16-byte, packed 8-byte and workspace 256-byte aligned", what);
+    return fail(ERR_UNSUPPORTED, "%s: base must be 16-byte, packed 8-byte and workspace 256-byte aligned", what);
   const int64_t rows = n * k / group;
+  const int64_t packed_rows = (rows + (8 / bits) - 1) / (8 / bits);
   const HqqLayout L = hqq_layout(rows, group, iters, 2);
+  char* ws = static_cast<char*>(workspace);
+  HqqHeader* header = reinterpret_cast<HqqHeader*>(ws);
+  double* partials = reinterpret_cast<double*>(ws + L.partials);
   HqqParams P;
   double b = beta;
   for (int i = 0; i < kHqqMaxIters; ++i) {
     P.inv_beta[i] = static_cast<float>(1.0 / b);
     b *= kappa;
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (cudaMemsetAsync(workspace, 0, sizeof(HqqHeader), st) != cudaSuccess)
-    return set_error(ERR_CUDA, "%s: memset failed", what);
-  const bool lp1 = lp_norm == 1.0;
   const double numel = static_cast<double>(n) * static_cast<double>(k);
-  const int tl = hqq_team_lanes(group);
-  char* ws = static_cast<char*>(workspace);
-  const bool zp = zeropoint != 0;
-  if (dtype == DT_BF16) {
-    const double e = hqq_pow_exponent<__nv_bfloat16>(lp_norm);
-    if (bits == 4) launch_hqq_bits<__nv_bfloat16, 4>(tl, base, packed, scale, shift, errors, ws, L, rows, group, zp, lp1, iters, e, numel, P, st);
-    else launch_hqq_bits<__nv_bfloat16, 2>(tl, base, packed, scale, shift, errors, ws, L, rows, group, zp, lp1, iters, e, numel, P, st);
-  } else {
-    const double e = hqq_pow_exponent<__half>(lp_norm);
-    if (bits == 4) launch_hqq_bits<__half, 4>(tl, base, packed, scale, shift, errors, ws, L, rows, group, zp, lp1, iters, e, numel, P, st);
-    else launch_hqq_bits<__half, 2>(tl, base, packed, scale, shift, errors, ws, L, rows, group, zp, lp1, iters, e, numel, P, st);
-  }
-  const cudaError_t err = cudaGetLastError();
-  return err == cudaSuccess ? OK : set_error(ERR_CUDA, "%s: launch failed: %s", what, cudaGetErrorString(err));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  rc = check_cuda(cudaMemsetAsync(workspace, 0, sizeof(HqqHeader), st), "quantize_qbits_hqq: workspace memset");
+  if (rc != OK) return rc;
+  return dispatch_act16(dtype, [&](auto act) {
+    return dispatch_bits(bits, [&](auto BITS) {
+      return dispatch_team_lanes(group, [&](auto TL) {
+        using T = typename decltype(act)::WT;
+        T* cands = reinterpret_cast<T*>(ws + L.cands);
+        auto search = [&](auto LP1) {
+          auto kern = hqq_search_kernel<T, BITS, TL, LP1>;
+          const int smem = table_smem<T, LP1>();
+          const int set = opt_into_table(kern, smem, "quantize_qbits_hqq: cudaFuncSetAttribute");
+          if (set != OK) return set;
+          kern<<<hqq_search_grid(rows, group), kHqqThreads, smem, st>>>(
+              static_cast<const T*>(base), static_cast<T*>(scale), cands, partials, header, errors, rows, group, iters,
+              hqq_pow_exponent<T>(lp_norm), numel, P);
+          return check_cuda(cudaGetLastError(), "quantize_qbits_hqq search launch");
+        };
+        const int searched = lp_norm == 1.0 ? search(std::true_type{}) : search(std::false_type{});
+        if (searched != OK) return searched;
+        return dispatch_zp(zeropoint, [&](auto ZP) {
+          hqq_pack_kernel<T, BITS, ZP, TL><<<capped_grid(packed_rows, kHqqThreads / TL, 8), kHqqThreads, 0, st>>>(
+              static_cast<const T*>(base), packed, static_cast<const T*>(scale), shift, cands, header, rows,
+              packed_rows, group);
+          return check_cuda(cudaGetLastError(), "quantize_qbits_hqq pack launch");
+        });
+      });
+    });
+  });
 }
 
 int qb200_hqq_shrink(const void* x, void* out, int64_t numel, double beta, double lp_norm, int dtype, void* stream) {
   const char* what = "hqq_shrink";
-  if (numel < 0) return set_error(ERR_ARG, "%s: negative size", what);
+  if (numel < 0) return fail(ERR_ARG, "%s: negative size", what);
   const int rc = hqq_check_config(what, dtype, lp_norm);
   if (rc != OK) return rc;
   if (numel == 0) return OK;
-  if (!x || !out) return set_error(ERR_ARG, "%s: null buffer", what);
+  if (!x || !out) return fail(ERR_ARG, "%s: null buffer", what);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const float inv = static_cast<float>(1.0 / beta);
-  const bool lp1 = lp_norm == 1.0;
-  int64_t blocks = (numel + kHqqThreads - 1) / kHqqThreads;
-  blocks = blocks > kNumSMsH100 * 2 ? kNumSMsH100 * 2 : blocks;
-  const int grid = static_cast<int>(blocks);
-#define QB_SHRINK(TT)                                                                                                 \
-  do {                                                                                                                \
-    const double e = hqq_pow_exponent<TT>(lp_norm);                                                                   \
-    if (lp1) {                                                                                                        \
-      hqq_shrink_kernel<TT, true><<<grid, kHqqThreads, 0, st>>>(static_cast<const TT*>(x), static_cast<TT*>(out),     \
-                                                                numel, inv, e);                                       \
-    } else {                                                                                                          \
-      const int smem = kHqqTable * static_cast<int>(sizeof(TT));                                                      \
-      cudaFuncSetAttribute(hqq_shrink_kernel<TT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);          \
-      hqq_shrink_kernel<TT, false><<<grid, kHqqThreads, smem, st>>>(static_cast<const TT*>(x), static_cast<TT*>(out), \
-                                                                    numel, inv, e);                                   \
-    }                                                                                                                 \
-  } while (0)
-  if (dtype == DT_BF16) QB_SHRINK(__nv_bfloat16);
-  else QB_SHRINK(__half);
-#undef QB_SHRINK
-  const cudaError_t err = cudaGetLastError();
-  return err == cudaSuccess ? OK : set_error(ERR_CUDA, "%s: launch failed: %s", what, cudaGetErrorString(err));
+  const int grid = capped_grid(numel, kHqqThreads, 2);
+  return dispatch_act16(dtype, [&](auto act) {
+    using T = typename decltype(act)::WT;
+    auto shrink = [&](auto LP1) {
+      auto kern = hqq_shrink_kernel<T, LP1>;
+      const int smem = table_smem<T, LP1>();
+      const int set = opt_into_table(kern, smem, "hqq_shrink: cudaFuncSetAttribute");
+      if (set != OK) return set;
+      kern<<<grid, kHqqThreads, smem, st>>>(static_cast<const T*>(x), static_cast<T*>(out), numel, inv,
+                                           hqq_pow_exponent<T>(lp_norm));
+      return check_cuda(cudaGetLastError(), "hqq_shrink launch");
+    };
+    return lp_norm == 1.0 ? shrink(std::true_type{}) : shrink(std::false_type{});
+  });
 }
 
 }  // extern "C"

@@ -229,17 +229,12 @@ __global__ void __launch_bounds__(WARP ? kWarpThreads : kMaxThreads)
   }
 }
 
-// 8-bit code dtype, or kFloatIO when `code` is the float dtype itself -> std::integral_constant
+// the input or output dtype `io`: kFloatIO when it is the float dtype itself, else an 8-bit code dtype ->
+// std::integral_constant
 template <class F>
-int dispatch_ln_io(int code, int dtype, F&& f) {
-  if (code == dtype) return f(std::integral_constant<int, kFloatIO>{});
-  switch (code) {
-    case DT_I8: return f(std::integral_constant<int, DT_I8>{});
-    case DT_E4M3: return f(std::integral_constant<int, DT_E4M3>{});
-    case DT_E5M2: return f(std::integral_constant<int, DT_E5M2>{});
-    case DT_E4M3FNUZ: return f(std::integral_constant<int, DT_E4M3FNUZ>{});
-    default: return fail(ERR_ARG, "layer_norm: dtype %d is neither the float dtype nor an 8-bit code dtype", code);
-  }
+int dispatch_ln_io(int io, int dtype, F&& f) {
+  if (io == dtype) return f(std::integral_constant<int, kFloatIO>{});
+  return dispatch_code8(io, f);
 }
 
 // threads of the CTA that owns a row of nvec 8-element chunks: enough to keep the row in registers, at most kMaxThreads
@@ -248,35 +243,6 @@ inline int ln_cta_threads(int64_t nvec) {
   const int64_t t = (per + 31) / 32 * 32;
   return static_cast<int>(t < 64 ? 64 : (t > kMaxThreads ? kMaxThreads : t));
 }
-
-template <typename T>
-static int launch_layer_norm(const void* x, const void* in_scale, const void* weight, const void* bias,
-                             const void* out_scale, bool out_scale_f32, void* out, int64_t rows, int64_t h, float eps,
-                             int in_dtype, int dtype, int out_dtype, cudaStream_t st) {
-  const int64_t nvec = (h + 7) / 8;
-  const bool vec = h % 8 == 0 && aligned16(x) && aligned16(out) && (weight == nullptr || aligned16(weight)) &&
-                   (bias == nullptr || aligned16(bias));
-  const bool warp = nvec <= 32 * kCacheVecs;
-  const int threads = warp ? kWarpThreads : ln_cta_threads(nvec);
-  const int64_t ctas = warp ? (rows + kWarpThreads / 32 - 1) / (kWarpThreads / 32) : rows;
-  const unsigned grid = static_cast<unsigned>(ctas < (1 << 20) ? ctas : (1 << 20));
-  const auto* sp = static_cast<const T*>(in_scale);
-  const auto* gp = static_cast<const T*>(weight);
-  const auto* bp = static_cast<const T*>(bias);
-  return dispatch_ln_io(in_dtype, dtype, [&](auto IN) {
-    return dispatch_ln_io(out_dtype, dtype, [&](auto OUT) {
-      if (warp)
-        layernorm_kernel<T, IN.value, OUT.value, true><<<grid, threads, 0, st>>>(
-            x, sp, gp, bp, out_scale, out_scale_f32, out, rows, static_cast<int>(h), eps, vec);
-      else
-        layernorm_kernel<T, IN.value, OUT.value, false><<<grid, threads, 0, st>>>(
-            x, sp, gp, bp, out_scale, out_scale_f32, out, rows, static_cast<int>(h), eps, vec);
-      return check_cuda(cudaGetLastError(), "layer_norm launch");
-    });
-  });
-}
-
-static bool is_code(int dt) { return dt == DT_I8 || dt == DT_E4M3 || dt == DT_E5M2 || dt == DT_E4M3FNUZ; }
 
 }  // namespace qb
 
@@ -290,11 +256,10 @@ int qb200_layer_norm(const void* x, const void* in_scale, const void* weight, co
   set_kernel_family(0);
   if (rows < 0 || h <= 0 || h > INT32_MAX) return fail(ERR_ARG, "layer_norm: bad shape (rows %lld, H %lld)",
                                                        static_cast<long long>(rows), static_cast<long long>(h));
-  if (dtype != DT_F32 && dtype != DT_F16 && dtype != DT_BF16)
-    return fail(ERR_ARG, "layer_norm: dtype must be F32, F16 or BF16 (got %d)", dtype);
-  if (in_dtype != dtype && !is_code(in_dtype))
+  if (!is_float_dtype(dtype)) return fail(ERR_ARG, "layer_norm: dtype must be F32, F16 or BF16 (got %d)", dtype);
+  if (in_dtype != dtype && !is_code_dtype(in_dtype))
     return fail(ERR_ARG, "layer_norm: input dtype %d is neither the float dtype nor an 8-bit code dtype", in_dtype);
-  if (out_dtype != dtype && !is_code(out_dtype))
+  if (out_dtype != dtype && !is_code_dtype(out_dtype))
     return fail(ERR_ARG, "layer_norm: output dtype %d is neither the float dtype nor an 8-bit code dtype", out_dtype);
   if (in_dtype != dtype && in_scale == nullptr) return fail(ERR_ARG, "layer_norm: codes in need their scale");
   if (out_dtype != dtype) {
@@ -304,20 +269,36 @@ int qb200_layer_norm(const void* x, const void* in_scale, const void* weight, co
   }
   if (!(eps >= 0.0)) return fail(ERR_ARG, "layer_norm: eps must be >= 0");
   if (rows == 0) return OK;
-  int rc = check_arch();
+  int rc = check_arch("layer_norm");
   if (rc != OK) return rc;
   set_kernel_family(6);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const bool f32_scale = out_scale_dtype == DT_F32;
+  const bool out_scale_f32 = out_scale_dtype == DT_F32;
   const float e = static_cast<float>(eps);
-  if (dtype == DT_BF16)
-    return launch_layer_norm<__nv_bfloat16>(x, in_scale, weight, bias, out_scale, f32_scale, out, rows, h, e, in_dtype,
-                                            dtype, out_dtype, st);
-  if (dtype == DT_F16)
-    return launch_layer_norm<__half>(x, in_scale, weight, bias, out_scale, f32_scale, out, rows, h, e, in_dtype, dtype,
-                                     out_dtype, st);
-  return launch_layer_norm<float>(x, in_scale, weight, bias, out_scale, f32_scale, out, rows, h, e, in_dtype, dtype,
-                                  out_dtype, st);
+  const int64_t nvec = (h + 7) / 8;
+  const bool vec = h % 8 == 0 && aligned16(x) && aligned16(out) && (weight == nullptr || aligned16(weight)) &&
+                   (bias == nullptr || aligned16(bias));
+  const bool warp = nvec <= 32 * kCacheVecs;
+  const int threads = warp ? kWarpThreads : ln_cta_threads(nvec);
+  const int64_t ctas = warp ? (rows + kWarpThreads / 32 - 1) / (kWarpThreads / 32) : rows;
+  const unsigned grid = static_cast<unsigned>(ctas < (1 << 20) ? ctas : (1 << 20));
+  return dispatch_float(dtype, [&](auto dt) {
+    return dispatch_ln_io(in_dtype, dtype, [&](auto IN) {
+      return dispatch_ln_io(out_dtype, dtype, [&](auto OUT) {
+        using T = typename decltype(dt)::T;
+        const auto* sp = static_cast<const T*>(in_scale);
+        const auto* gp = static_cast<const T*>(weight);
+        const auto* bp = static_cast<const T*>(bias);
+        if (warp)
+          layernorm_kernel<T, IN.value, OUT.value, true><<<grid, threads, 0, st>>>(
+              x, sp, gp, bp, out_scale, out_scale_f32, out, rows, static_cast<int>(h), e, vec);
+        else
+          layernorm_kernel<T, IN.value, OUT.value, false><<<grid, threads, 0, st>>>(
+              x, sp, gp, bp, out_scale, out_scale_f32, out, rows, static_cast<int>(h), e, vec);
+        return check_cuda(cudaGetLastError(), "layer_norm launch");
+      });
+    });
+  });
 }
 
 }  // extern "C"
